@@ -29,6 +29,10 @@ struct StreamJob {
     uint32_t       symbolic;    // 1: dst is uint16_t[dst_cap]; a byte copied from in front of the segment becomes
                                 // the marker 0x8000 | index into the 32 KiB window that precedes the segment
     uint32_t       pad_;
+    // host-side planning only (no kernel reads them): a device buffer of `scratch_cap` bytes that is dead while the
+    // stream is inflated (the image's pixel buffer, written by unfilter afterwards), or null
+    uint8_t*       scratch;
+    uint64_t       scratch_cap;
 };
 
 struct StreamResult {

@@ -18,6 +18,7 @@
 #pragma once
 
 #include "common.cuh"
+#include "inflate_wave.cuh"
 
 namespace pngb200 {
 
@@ -81,6 +82,117 @@ __global__ void __launch_bounds__(256) marker_resolve_kernel(const SegmentRecord
         const uint16_t x = s.sym[i];
         s.out[i] = (x & 0x8000u) ? (s.first ? 0 : w[x & 0x7fffu]) : (uint8_t)x;
     }
+}
+
+// ---- a stream cut in two (DESIGN.md section 4.2 "head and tail") ----
+// The HEAD decodes bits [0, split) straight into the stream's output and folds Adler-32 as a whole stream does;
+// the TAIL decodes from the block header at `split` to the trailer into symbols.  The 32 KiB in front of the tail
+// is the end of the head's output, already final, so no window chain is needed: one pass replaces the markers,
+// writes the tail's bytes behind the head's and folds their Adler-32 partial sums.
+struct SplitRecord {
+    const StreamResult* head;      // head's result: produced = n1, checksum = Adler-32 of bytes [0, n1)
+    const StreamResult* tail;      // tail's result: produced = n2, declared = the stream's trailer
+    const uint16_t*     sym;       // the tail's symbols
+    uint8_t*            out;       // the stream's output (the head's dst)
+    uint64_t            dst_cap;
+    uint64_t            split_bit; // where the tail starts (the head's stop_bit)
+    StreamResult*       final_;    // the stream's result record, written only when the split is accepted
+};
+
+constexpr uint32_t SPLIT_CTAS = 64;  // resolve CTAs per split stream (blockIdx.y)
+
+// the pieces line up: the head ended on the tail's first block header, the tail reached the trailer, and the
+// head is long enough to hold every byte a marker can refer to
+__device__ __forceinline__ bool split_lines_up(const SplitRecord& s, uint64_t n1, uint64_t n2)
+{
+    return s.head->status == PNGB200_OK && s.head->phase == 1 && s.head->consumed_bits == s.split_bit &&
+           s.tail->status == PNGB200_OK && s.tail->phase == 2 && n1 >= SEG_WINDOW && n1 + n2 <= s.dst_cap;
+}
+
+// grid (splits, SPLIT_CTAS): CTA y takes the 4096-symbol chunks y, y + SPLIT_CTAS, ... of its stream's tail and
+// leaves the tail's Adler-32 partial sums (sum of b, sum of (n2 - i) b, both mod 65521) in partial[2 * (k * SPLIT_CTAS + y)]
+__global__ void __launch_bounds__(256) split_resolve_kernel(const SplitRecord* recs, uint32_t* partial)
+{
+    const SplitRecord s  = recs[blockIdx.x];
+    const uint64_t    n1 = s.head->produced, n2 = s.tail->produced;
+    uint32_t*         pp = partial + 2 * ((size_t)blockIdx.x * SPLIT_CTAS + blockIdx.y);
+    if (!split_lines_up(s, n1, n2)) return;
+    const uint8_t* w = s.out + n1 - SEG_WINDOW;   // marker index -> byte in front of the tail
+    uint8_t*       o = s.out + n1;
+    uint64_t a = 0, b = 0;
+    for (uint64_t base = (uint64_t)blockIdx.y * 4096; base < n2; base += (uint64_t)SPLIT_CTAS * 4096) {
+        for (uint32_t j = threadIdx.x; j < 4096; j += blockDim.x) {
+            const uint64_t i = base + j;
+            if (i >= n2) break;
+            const uint16_t x = s.sym[i];
+            const uint8_t  v = (x & 0x8000u) ? w[x & 0x7fffu] : (uint8_t)x;
+            o[i] = v;
+            a += v;
+            b += (n2 - i) * v;
+        }
+        b %= ADLER_MOD32;
+    }
+    uint32_t a32 = (uint32_t)(a % ADLER_MOD32), b32 = (uint32_t)b;
+    for (int k = 16; k; k >>= 1) {
+        a32 += __shfl_down_sync(0xffffffffu, a32, k);
+        b32 += __shfl_down_sync(0xffffffffu, b32, k);
+    }
+    __shared__ uint32_t red[2][8];
+    const unsigned warp = threadIdx.x >> 5;
+    if (lane_id() == 0) { red[0][warp] = a32 % ADLER_MOD32; red[1][warp] = b32 % ADLER_MOD32; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t sa = 0, sb = 0;
+        for (unsigned k = 0; k < blockDim.x / 32; ++k) { sa += red[0][k]; sb += red[1][k]; }
+        pp[0] = sa % ADLER_MOD32;
+        pp[1] = sb % ADLER_MOD32;
+    }
+}
+
+// one thread per split stream: Adler-32 of head ++ tail from the head's checksum and the tail's partial sums, checked
+// against the trailer.  A stream whose pieces line up and whose checksum matches gets its final result record and
+// accept[k] = 1; any other stream keeps an untouched record (accept[k] = 0) and is decoded whole afterwards.
+__global__ void __launch_bounds__(128) split_finish_kernel(const SplitRecord* recs, uint32_t count, const uint32_t* partial,
+                                                           uint32_t* accept)
+{
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= count) return;
+    const SplitRecord s  = recs[k];
+    const uint64_t    n1 = s.head->produced, n2 = s.tail->produced;
+    bool ok = split_lines_up(s, n1, n2) && s.head->ck_done;
+    uint32_t computed = 0;
+    if (ok) {
+        uint64_t ta = 0, tb = 0;
+        for (uint32_t y = 0; y < SPLIT_CTAS; ++y) {
+            ta += partial[2 * ((size_t)k * SPLIT_CTAS + y)];
+            tb += partial[2 * ((size_t)k * SPLIT_CTAS + y) + 1];
+        }
+        // adler(H ++ T): A = A_H + sum T, B = B_H + |T| A_H + sum (|T| - i) T_i  (the zlib adler32_combine arithmetic)
+        const uint64_t ah = s.head->checksum & 0xffffu, bh = s.head->checksum >> 16;
+        const uint64_t A = (ah + ta) % ADLER_MOD32;
+        const uint64_t B = (bh + (n2 % ADLER_MOD32) * ah + tb) % ADLER_MOD32;
+        computed = (uint32_t)(B << 16 | A);
+        ok = computed == s.tail->declared;
+    }
+    accept[k] = ok ? 1u : 0u;
+    if (!ok) return;
+    // what a whole-stream decode reports: trailer fields from the tail, counts over both pieces
+    StreamResult f = *s.tail;
+    const StreamResult& h = *s.head;
+    f.produced   = n1 + n2;
+    f.resume_out = n1 + f.resume_out;
+    f.blocks     = h.blocks + f.blocks;
+    f.checksum   = computed;
+    f.ck_done    = 1;
+    f.stat_waves += h.stat_waves;
+    f.stat_sync_rounds += h.stat_sync_rounds;
+    f.stat_resolve_rounds = max(f.stat_resolve_rounds, h.stat_resolve_rounds);
+    f.stat_fallback |= h.stat_fallback;
+    f.stat_tokens += h.stat_tokens;
+    f.stat_matches += h.stat_matches;
+    f.stat_deferred += h.stat_deferred;
+    for (int q = 0; q < 12; ++q) f.stat_cycles[q] += h.stat_cycles[q];
+    *s.final_ = f;
 }
 
 }  // namespace pngb200

@@ -115,6 +115,9 @@ struct pngb200_ctx {
     size_t parallel_threshold = 8192;  // streams at least this long use the block-parallel kernel
     unsigned long long* d_hist = nullptr;   // filter-type histogram of the last wavefront-unfilter launch (in d_imgjobs)
     size_t peer_streams = 0;           // lanes: streams of the whole host batch (its chunks run side by side on this GPU)
+    bool   split = true;               // cut big streams into a head and a tail when that evens out the CTA slots (PNGB200_SPLIT=0: off)
+    size_t plan_slots = 0;             // CTA slots the segment and split planners assume, 0 = the ring kernel's (PNGB200_PLAN_SLOTS:
+                                       // lets a small test batch take the paths meant for a full GPU)
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // decode stage boundaries
     // geometry of the pending decode batch
     std::vector<uint64_t> expected;   // filtered bytes expected per image
@@ -373,6 +376,144 @@ int run_segments(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t
     return PNGB200_OK;
 }
 
+// CTA slots the segment and split planners fill
+size_t plan_slots(const pngb200_ctx* ctx) { return ctx->plan_slots ? ctx->plan_slots : (size_t)ctx->sm_count * WV_CTAS_PER_SM; }
+
+// ---- a stream cut in two: a direct head and a symbolic tail (inflate_segments.cuh, DESIGN.md section 4.2) ----
+// Per output byte, inflate_wave_kernel in symbolic mode (tails) costs this many times what it costs writing bytes
+// (heads): stat_cycles over produced, 13.8 against 10.0 cycles per byte, for the 198 x 7680x4320 RGBA8 photo batch
+// (bench.py's default) cut at h = 0.78, on an H100 80GB HBM3 at a 400 W power limit and 1980 MHz.
+constexpr double kSymbolicCost = 1.38;
+
+// B big streams on N CTA slots with N / 2 < B < N: one CTA per stream would leave N - B slots idle for the whole
+// launch.  Each stream is cut at a block boundary instead: heads take the first B tickets, the N - B other CTAs
+// work through the tails one after another.  Head share h = B rho / (N - B + B rho) gives a chain of B / (N - B)
+// tails the cost of one head.  The tail's symbols go to the stream's scratch (the image's pixel buffer, dead until
+// unfilter); the head's bytes are final where they land.  On return `par` holds the streams still to be decoded
+// whole: not cut, or cut but not accepted (split_finish_kernel) -- so statuses and errors are those of the
+// whole-stream path for every input.
+
+// the head share h when the big streams `par` are to be cut, else 0
+double split_head_share(const pngb200_ctx* ctx, const StreamJob* h_jobs, const std::vector<uint32_t>& par)
+{
+    constexpr uint64_t kMinSplit = 1u << 20;   // compressed bytes of a stream worth cutting, at least
+    const size_t slots = plan_slots(ctx), nb = par.size();
+    if (!ctx->split || ctx->peer_streams || nb * 2 <= slots || nb >= slots) return 0;
+    const double h = nb * kSymbolicCost / ((double)(slots - nb) + nb * kSymbolicCost);
+    if (h < 0.55 || h > 0.95) return 0;   // below: the tail would not fit its scratch; above: little to gain
+    for (uint32_t i : par) {   // every big stream qualifies, or none is cut (a second launch would serialise them)
+        const StreamJob& j = h_jobs[i];
+        if (j.format != PNGB200_FORMAT_ZLIB || j.start_bit != 0 || j.phase != 0 || j.src_len < kMinSplit || j.dst_cap < kMinSplit ||
+            !j.scratch || (uintptr_t)j.scratch % 16 || (double)j.scratch_cap < 2.5 * (1.0 - h) * (double)j.dst_cap + 4096)
+            return 0;
+    }
+    return h;
+}
+
+int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& par, double h)
+{
+    const size_t slots = plan_slots(ctx), nb = par.size();
+    // 1. split points: the first plausible dynamic-block header at or after h of the stream
+    CU(ctx->h_sgsearch.reserve(sizeof(SearchJob) * nb));
+    CU(ctx->d_sgsearch.reserve(sizeof(SearchJob) * nb));
+    SearchJob* sj = ctx->h_sgsearch.as<SearchJob>();
+    for (size_t k = 0; k < nb; ++k) {
+        const StreamJob& j = h_jobs[par[k]];
+        sj[k] = SearchJob{j.src, j.src_len, (uint64_t)(h * (double)(8 * j.src_len)), 8 * j.src_len, ~0ull};
+    }
+    CU(cudaMemcpyAsync(ctx->d_sgsearch.p, sj, sizeof(SearchJob) * nb, cudaMemcpyHostToDevice, ctx->stream));
+    block_search_kernel<<<dim3((unsigned)nb, BS_CTAS), 256, 0, ctx->stream>>>(ctx->d_sgsearch.as<SearchJob>(), (uint32_t)nb);
+    ctx->launches++;
+    CU(cudaMemcpyAsync(sj, ctx->d_sgsearch.p, sizeof(SearchJob) * nb, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    // 2. heads (LPT order, first tickets), then the tails in the same order
+    std::vector<uint32_t> cut, rest;
+    for (size_t k = 0; k < nb; ++k) (sj[k].found != ~0ull ? cut : rest).push_back(par[k]);
+    const size_t n = cut.size();
+    if (n == 0) return PNGB200_OK;
+    CU(ctx->h_sgjobs.reserve(sizeof(StreamJob) * 2 * n));
+    CU(ctx->d_sgjobs.reserve(sizeof(StreamJob) * 2 * n));
+    CU(ctx->d_sgres.reserve(sizeof(StreamResult) * 2 * n));
+    StreamJob* sg = ctx->h_sgjobs.as<StreamJob>();
+    uint64_t max_cap = 0;
+    for (size_t k = 0, s = 0; k < nb; ++k) {
+        if (sj[k].found == ~0ull) continue;
+        const StreamJob& j = h_jobs[par[k]];
+        StreamJob& hd = sg[s];
+        StreamJob& tl = sg[n + s];
+        ++s;
+        hd = j;
+        hd.stop_bit = sj[k].found;
+        tl = j;
+        tl.start_bit = sj[k].found;
+        tl.phase = 1;
+        tl.symbolic = 1;
+        tl.dst = j.scratch;
+        tl.dst_cap = j.scratch_cap / 2 - 64;   // symbols, with the kernel's store slack behind them
+        max_cap = std::max(max_cap, j.dst_cap);
+    }
+    CU(cudaMemcpyAsync(ctx->d_sgjobs.p, sg, sizeof(StreamJob) * 2 * n, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemsetAsync(ctx->d_sgres.p, 0, sizeof(StreamResult) * 2 * n, ctx->stream));
+    {
+        WvParams pp;
+        pp.bitmap_words = wv_bitmap_words(max_cap);
+        pp.scratch_stride = wv_scratch_stride(pp.bitmap_words);
+        const unsigned grid = (unsigned)std::min<size_t>(2 * n, slots);
+        const size_t need = (size_t)pp.scratch_stride * grid + 256;
+        if (need > ctx->d_scratch.cap || pp.scratch_stride != ctx->scratch_stride) {   // bitmaps start zeroed (see run_inflate)
+            CU(ctx->d_scratch.reserve(need));
+            CU(cudaMemsetAsync(ctx->d_scratch.p, 0, ctx->d_scratch.cap, ctx->stream));
+            ctx->scratch_stride = pp.scratch_stride;
+        }
+        pp.ticket = (uint32_t*)((char*)ctx->d_scratch.p + (size_t)pp.scratch_stride * grid);
+        CU(cudaMemsetAsync(pp.ticket, 0, sizeof(uint32_t), ctx->stream));
+        pp.jobs = ctx->d_sgjobs.as<StreamJob>();
+        pp.results = ctx->d_sgres.as<StreamResult>();
+        pp.order = nullptr;
+        pp.scratch = ctx->d_scratch.as<uint8_t>();
+        pp.count = (int)(2 * n);
+        inflate_wave_kernel<<<grid, WV_THREADS, sizeof(WvShared), ctx->stream>>>(pp);
+        ctx->launches++;
+    }
+    // 3. tails -> bytes behind their heads, Adler-32 of the whole stream, acceptance; device-side, one host round trip
+    const size_t off_accept  = align_up(sizeof(SplitRecord) * n, 256);
+    const size_t off_partial = align_up(off_accept + sizeof(uint32_t) * n, 256);
+    const size_t table       = off_partial + sizeof(uint32_t) * 2 * SPLIT_CTAS * n;
+    CU(ctx->h_sgrec.reserve(off_partial));
+    CU(ctx->d_sgrec.reserve(table));
+    SplitRecord* rec = ctx->h_sgrec.as<SplitRecord>();
+    const StreamResult* d_sgres = ctx->d_sgres.as<StreamResult>();
+    for (size_t s = 0; s < n; ++s) {
+        const StreamJob& j = h_jobs[cut[s]];
+        rec[s] = SplitRecord{d_sgres + s, d_sgres + n + s, (const uint16_t*)j.scratch, j.dst, j.dst_cap, sg[s].stop_bit,
+                             ctx->d_results.as<StreamResult>() + cut[s]};
+    }
+    CU(cudaMemcpyAsync(ctx->d_sgrec.p, rec, sizeof(SplitRecord) * n, cudaMemcpyHostToDevice, ctx->stream));
+    const SplitRecord* d_rec = ctx->d_sgrec.as<SplitRecord>();
+    uint32_t* d_accept  = (uint32_t*)((char*)ctx->d_sgrec.p + off_accept);
+    uint32_t* d_partial = (uint32_t*)((char*)ctx->d_sgrec.p + off_partial);
+    split_resolve_kernel<<<dim3((unsigned)n, SPLIT_CTAS), 256, 0, ctx->stream>>>(d_rec, d_partial);
+    split_finish_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(d_rec, (uint32_t)n, d_partial, d_accept);
+    ctx->launches += 2;
+    CU(cudaGetLastError());
+    uint32_t* accept = (uint32_t*)((char*)ctx->h_sgrec.p + off_accept);
+    CU(cudaMemcpyAsync(accept, d_accept, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    ctx->seg_streams += n;
+    ctx->seg_segments += 2 * n;
+    for (size_t s = 0; s < n; ++s)
+        if (!accept[s]) {
+            ctx->seg_fallbacks++;
+            rest.push_back(cut[s]);
+        }
+    // what is left keeps its longest-first order
+    std::vector<uint32_t> left;
+    for (uint32_t i : par)
+        if (std::find(rest.begin(), rest.end(), i) != rest.end()) left.push_back(i);
+    par.swap(left);
+    return PNGB200_OK;
+}
+
 // ---- inflate (+ checksum) over a device-resident job table ----
 // h_jobs: host copy (for dst_cap based chunk layout); d_jobs/d_results device arrays of `count`.
 int run_inflate(pngb200_ctx* ctx, const StreamJob* h_jobs, size_t count)
@@ -414,10 +555,14 @@ int run_inflate(pngb200_ctx* ctx, const StreamJob* h_jobs, size_t count)
         if (ctx->inflate_mode == 0 || ctx->inflate_mode == 5) {
             // few big streams: cut them so that every CTA slot has something to decode
             const size_t before = par.size();
-            if (!par.empty() && std::max(par.size(), ctx->peer_streams) * 2 <= (size_t)ctx->sm_count * WV_CTAS_PER_SM) {
+            if (!par.empty() && std::max(par.size(), ctx->peer_streams) * 2 <= plan_slots(ctx)) {
                 if (int rc = before_first_launch()) return rc;
                 hooked = true;
                 if (int rc = run_segments(ctx, h_jobs, par)) return rc;
+            } else if (const double h = split_head_share(ctx, h_jobs, par)) {
+                if (int rc = before_first_launch()) return rc;
+                hooked = true;
+                if (int rc = run_split(ctx, h_jobs, par, h)) return rc;
             }
             if (par.size() != before) {   // the order table lists what is left for the whole-stream kernels
                 std::copy(par.begin(), par.end(), ho);
@@ -836,6 +981,8 @@ pngb200_ctx* pngb200_ctx_create(int device)
     ctx->device_bytes = prop.totalGlobalMem;
     if (const char* v = getenv("PNGB200_CELLS_AUTO")) ctx->cells_auto = atoi(v) != 0;   // tuning overrides, read once per context
     if (const char* v = getenv("PNGB200_CELLS_SEGMENTS")) ctx->cells_segments = atoi(v) != 0;
+    if (const char* v = getenv("PNGB200_SPLIT")) ctx->split = atoi(v) != 0;
+    if (const char* v = getenv("PNGB200_PLAN_SLOTS")) ctx->plan_slots = (size_t)std::max(0, atoi(v));
     DeviceGuard guard(device);
     if (cudaFuncSetAttribute(deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DfShared)) != cudaSuccess) {
         set_error(nullptr, PNGB200_ERR_CUDA, "cannot opt in to %zu bytes of shared memory", sizeof(DfShared));
@@ -1032,6 +1179,8 @@ int pngb200_inflate_batch(pngb200_ctx* ctx, pngb200_stream_desc* s, size_t count
         jobs[i].stop_bit = 0;
         jobs[i].symbolic = 0;
         jobs[i].pad_ = 0;
+        jobs[i].scratch = nullptr;   // no buffer to borrow: streams are not cut in two
+        jobs[i].scratch_cap = 0;
     }
     CU(cudaMemcpyAsync(ctx->d_jobs.p, jobs, sizeof(StreamJob) * count, cudaMemcpyHostToDevice, ctx->stream));
     int rc = run_inflate(ctx, jobs, count);
@@ -1115,6 +1264,10 @@ int pngb200_decode_batch_enqueue(pngb200_ctx* ctx, pngb200_image_desc* im, size_
         jobs[i].stop_bit = 0;
         jobs[i].symbolic = 0;
         jobs[i].pad_ = 0;
+        // the pixel buffer is dead until unfilter writes it: a stream cut in two keeps its tail's symbols there
+        // (host batches run lanes side by side and are not cut)
+        jobs[i].scratch = host ? nullptr : im[i].pixels;
+        jobs[i].scratch_cap = host ? 0 : im[i].pixels_cap;
     }
     CU(cudaMemcpyAsync(ctx->d_jobs.p, jobs, sizeof(StreamJob) * count, cudaMemcpyHostToDevice, ctx->stream));
     int rc = run_inflate(ctx, jobs, count);
