@@ -139,6 +139,11 @@ int          pngb200_ctx_inflate_counters(pngb200_ctx* ctx, size_t count, uint64
  * decode batch on this context: out[0] streams that were cut, out[1] segments they were cut into, out[2] streams
  * whose segments did not line up and that were decoded whole after all (results are identical either way). */
 int          pngb200_ctx_segment_stats(pngb200_ctx* ctx, uint64_t out[3]);
+/* streams of the last inflate / decode batch that were cut into a direct head and a symbolic tail and accepted:
+ * out[0] heads' bytes, out[1] heads' SM cycles (thread 0 of the CTA, all phases), out[2] tails' bytes, out[3]
+ * tails' SM cycles, out[4] tails that left symbolic mode once their last 32 KiB held no marker, out[5] tails'
+ * bytes decoded as symbols */
+int          pngb200_ctx_split_stats(pngb200_ctx* ctx, uint64_t out[6]);
 /* which whole-stream engine the last inflate / decode batch on this context launched: 0 inflate_parallel_kernel
  * (round 1), 1 inflate_wave_kernel (ring window), 2 inflate_cells_kernel, -1 none (tiny streams, segments only) */
 int          pngb200_ctx_last_inflate_engine(pngb200_ctx* ctx);

@@ -236,6 +236,9 @@ def lib():
     L.pngb200_ctx_filter_histogram.restype = C.c_int
     L.pngb200_ctx_segment_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.pngb200_ctx_segment_stats.restype = C.c_int
+    if os.environ.get("PNGB200_LIB") is None or hasattr(L, "pngb200_ctx_split_stats"):   # (older tuning builds lack it)
+        L.pngb200_ctx_split_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.pngb200_ctx_split_stats.restype = C.c_int
     if os.environ.get("PNGB200_LIB") is None or hasattr(L, "pngb200_ctx_last_inflate_engine"):   # (older tuning builds lack it)
         L.pngb200_ctx_last_inflate_engine.argtypes = [C.c_void_p]
         L.pngb200_ctx_last_inflate_engine.restype = C.c_int
@@ -358,6 +361,14 @@ class Context:
         out = (C.c_uint64 * 3)()
         self.check(self._lib.pngb200_ctx_segment_stats(self.handle, out))
         return dict(streams=out[0], segments=out[1], fallbacks=out[2])
+
+    def split_stats(self):
+        """bytes and SM cycles of the heads and tails of the streams the last batch cut in two, the tails that left
+        symbolic mode and the tails' bytes decoded as symbols (see pngb200_ctx_split_stats)"""
+        out = (C.c_uint64 * 6)()
+        self.check(self._lib.pngb200_ctx_split_stats(self.handle, out))
+        return dict(head_bytes=out[0], head_cycles=out[1], tail_bytes=out[2], tail_cycles=out[3], switched=out[4],
+                    symbolic_bytes=out[5])
 
     def last_inflate_engine(self) -> str:
         """kernel name of the whole-stream inflate engine the last batch used ('' when none ran)"""

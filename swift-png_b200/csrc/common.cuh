@@ -28,7 +28,8 @@ struct StreamJob {
     uint64_t       stop_bit;    // 0 = to the end of the stream; else stop at the first block boundary >= stop_bit
     uint32_t       symbolic;    // 1: dst is uint16_t[dst_cap]; a byte copied from in front of the segment becomes
                                 // the marker 0x8000 | index into the 32 KiB window that precedes the segment
-    uint32_t       pad_;
+    uint32_t       may_switch;  // symbolic tails of a stream cut in two: once the last 32 KiB hold no marker, go on
+                                // in bytes behind the symbols (dst then holds 2 dst_cap bytes; SwitchRecord)
     // host-side planning only (no kernel reads them): a device buffer of `scratch_cap` bytes that is dead while the
     // stream is inflated (the image's pixel buffer, written by unfilter afterwards), or null
     uint8_t*       scratch;
@@ -55,6 +56,13 @@ struct StreamResult {
     // SM cycles thread 0 of the stream's CTA spent per phase of the wave kernel (each ends at a barrier):
     // 0 header+tables 1 stage 2 speculate 3 walk 4 chain 5 count+scan 6 emit 7 resolve 8 store 9 stored blocks
     uint64_t stat_cycles[12];
+};
+
+// Where a symbolic job with may_switch left symbolic mode (inflate_wave_kernel, WvParams.switched): output [0, out)
+// is symbols at dst, [out, produced) bytes that start at byte `bytes` of dst.  out = produced: it never switched.
+struct SwitchRecord {
+    uint64_t out;
+    uint64_t bytes;
 };
 
 // One image for the unfilter stage.

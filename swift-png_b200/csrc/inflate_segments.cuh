@@ -97,7 +97,11 @@ struct SplitRecord {
     uint64_t            dst_cap;
     uint64_t            split_bit; // where the tail starts (the head's stop_bit)
     StreamResult*       final_;    // the stream's result record, written only when the split is accepted
+    const SwitchRecord* sw = nullptr;   // where the tail left symbolic mode; null: it did not (all n2 are symbols)
 };
+
+// tail bytes [0, m) are symbols, [m, n2) bytes (SwitchRecord)
+__device__ __forceinline__ uint64_t split_switch_out(const SplitRecord& s, uint64_t n2) { return s.sw ? s.sw->out : n2; }
 
 constexpr uint32_t SPLIT_CTAS = 64;  // resolve CTAs per split stream (blockIdx.y)
 
@@ -106,29 +110,62 @@ constexpr uint32_t SPLIT_CTAS = 64;  // resolve CTAs per split stream (blockIdx.
 __device__ __forceinline__ bool split_lines_up(const SplitRecord& s, uint64_t n1, uint64_t n2)
 {
     return s.head->status == PNGB200_OK && s.head->phase == 1 && s.head->consumed_bits == s.split_bit &&
-           s.tail->status == PNGB200_OK && s.tail->phase == 2 && n1 >= SEG_WINDOW && n1 + n2 <= s.dst_cap;
+           s.tail->status == PNGB200_OK && s.tail->phase == 2 && n1 >= SEG_WINDOW && n1 + n2 <= s.dst_cap &&
+           split_switch_out(s, n2) <= n2;
 }
 
-// grid (splits, SPLIT_CTAS): CTA y takes the 4096-symbol chunks y, y + SPLIT_CTAS, ... of its stream's tail and
-// leaves the tail's Adler-32 partial sums (sum of b, sum of (n2 - i) b, both mod 65521) in partial[2 * (k * SPLIT_CTAS + y)]
+// grid (splits, SPLIT_CTAS): CTA y takes the 4096-byte chunks y, y + SPLIT_CTAS, ... of its stream's tail and leaves
+// the tail's Adler-32 partial sums (sum of b, sum of (n2 - i) b, both mod 65521) in partial[2 * (k * SPLIT_CTAS + y)].
+// Tail bytes [0, m) are symbols; [m, n2) are bytes the tail wrote after it left symbolic mode (SplitRecord.sw)
 __global__ void __launch_bounds__(256) split_resolve_kernel(const SplitRecord* recs, uint32_t* partial)
 {
     const SplitRecord s  = recs[blockIdx.x];
     const uint64_t    n1 = s.head->produced, n2 = s.tail->produced;
     uint32_t*         pp = partial + 2 * ((size_t)blockIdx.x * SPLIT_CTAS + blockIdx.y);
     if (!split_lines_up(s, n1, n2)) return;
+    const uint64_t m = split_switch_out(s, n2);
     const uint8_t* w = s.out + n1 - SEG_WINDOW;   // marker index -> byte in front of the tail
     uint8_t*       o = s.out + n1;
+    const uint8_t* bytes = reinterpret_cast<const uint8_t*>(s.sym) + (s.sw ? s.sw->bytes : 0);   // tail byte m
     uint64_t a = 0, b = 0;
     for (uint64_t base = (uint64_t)blockIdx.y * 4096; base < n2; base += (uint64_t)SPLIT_CTAS * 4096) {
-        for (uint32_t j = threadIdx.x; j < 4096; j += blockDim.x) {
-            const uint64_t i = base + j;
-            if (i >= n2) break;
+        const uint64_t end = min(base + 4096, n2);
+        for (uint64_t i = base + threadIdx.x; i < min(end, m); i += blockDim.x) {
             const uint16_t x = s.sym[i];
             const uint8_t  v = (x & 0x8000u) ? w[x & 0x7fffu] : (uint8_t)x;
             o[i] = v;
             a += v;
             b += (n2 - i) * v;
+        }
+        if (end > m) {
+            // bytes [lo, end): 16-byte stores aligned in the output; the source (any relative alignment) is read as
+            // five aligned words per store and shifted into place
+            const uint64_t  lo = max(base, m);
+            const uintptr_t g0 = (uintptr_t)(o + lo) & ~(uintptr_t)15;
+            const uint64_t  ng = ((uintptr_t)(o + end) - g0 + 15) / 16;
+            for (uint64_t g = threadIdx.x; g < ng; g += blockDim.x) {
+                const int64_t i0 = (int64_t)(g0 + 16 * g - (uintptr_t)o);   // tail offset of the group's first byte
+                if (i0 >= (int64_t)lo && (uint64_t)i0 + 16 <= end) {
+                    const uint8_t*  src = bytes + ((uint64_t)i0 - m);
+                    const uint32_t* sw  = reinterpret_cast<const uint32_t*>((uintptr_t)src & ~(uintptr_t)3);
+                    const uint32_t  sh  = 8 * (uint32_t)((uintptr_t)src & 3);
+                    const uint32_t  w0 = sw[0], w1 = sw[1], w2 = sw[2], w3 = sw[3], w4 = sw[4];
+                    uint4 x;
+                    x.x = __funnelshift_r(w0, w1, sh);
+                    x.y = __funnelshift_r(w1, w2, sh);
+                    x.z = __funnelshift_r(w2, w3, sh);
+                    x.w = __funnelshift_r(w3, w4, sh);
+                    *reinterpret_cast<uint4*>(o + i0) = x;
+                    adler_chunk16(x, n2 - (uint64_t)i0, a, b);
+                } else {
+                    for (int64_t i = max(i0, (int64_t)lo); i < min(i0 + 16, (int64_t)end); ++i) {
+                        const uint8_t v = bytes[i - m];
+                        o[i] = v;
+                        a += v;
+                        b += (n2 - i) * v;
+                    }
+                }
+            }
         }
         b %= ADLER_MOD32;
     }

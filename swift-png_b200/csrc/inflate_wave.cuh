@@ -131,6 +131,7 @@ struct WvShared {
     uint64_t     warp_sums[WV_WARPS + 1];
     uint32_t     adler_a[WV_WARPS], adler_b[WV_WARPS];
     uint32_t     exc[WV_WARPS], valid[WV_WARPS];
+    uint32_t     mark[WV_WARPS];                // symbolic wave: 1 + the last wave offset holding a marker, per warp
     uint32_t     last, term, anomaly, ticket;
     uint64_t     cyc[12], tick;                 // phase timers (thread 0)
     uint64_t     pf_bar;                        // mbarrier of the bulk prefetch (lands in mask[] .. ck[], dead by then)
@@ -146,6 +147,7 @@ struct WvParams {
     uint64_t         scratch_stride;
     uint64_t         bitmap_words; // size of the HBM bitmap of each CTA
     int              count;
+    SwitchRecord*    switched = nullptr;   // per job, or null: where a job with may_switch left symbolic mode
 };
 
 struct CopyItem { uint32_t o; uint32_t run_dist; };  // run | (dist - 1) << 16; run == 0: empty slot
@@ -704,11 +706,16 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
         int      st     = PNGB200_OK;
         uint32_t phase  = (uint32_t)job.phase;
         uint64_t resume_bit = job.start_bit, resume_out = job.start_out;
-        uint8_t* const dst = job.dst;
-        const bool     sym = job.symbolic != 0;       // segment: 16-bit symbols, always written straight to HBM
-        const uint32_t esz = sym ? 2u : 1u;
-        const uint32_t mis = (uint32_t)((uintptr_t)dst & 15);  // ring position = stream offset + mis (mod 65536)
-        bool fallback = false;
+        uint8_t* dst     = job.dst;
+        uint64_t dst_cap = job.dst_cap;
+        bool     sym     = job.symbolic != 0;         // segment: 16-bit symbols, always written straight to HBM
+        uint32_t esz     = sym ? 2u : 1u;
+        uint32_t mis     = (uint32_t)((uintptr_t)dst & 15);  // ring position = stream offset + mis (mod 65536)
+        // a tail that may leave symbolic mode: 1 + the last offset that holds a marker (tracked while symbolic), and
+        // where it switched (~0: it did not) / the byte offset in job.dst of its byte `sw_out`
+        const bool may_switch = sym && job.may_switch;
+        uint64_t   mark_end = 0, sw_out = ~0ull, sw_bytes = 0;
+        bool fallback = false, over_cap = false;
         bool ring_stale = job.start_out != 0;   // the ring does not hold the window [out - 32768, out)
         bool     pf_pending = false;            // a bulk prefetch is in flight / has landed
         uint64_t pf_first = 0;                  // first word (reader space) of the prefetched range
@@ -750,6 +757,28 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                 sh.cyc[i] += now - sh.tick;
                 sh.tick = now;
             }
+        };
+        // A symbolic tail whose last 32 KiB hold no marker: DEFLATE distances are at most 32768, so no later byte can
+        // depend on the output in front of the tail, and the rest is decoded as a head decodes it.  The window goes,
+        // as bytes, in front of a byte area behind the symbols, so that the ring refill (ring_stale), oversized waves
+        // and stored blocks find it where a direct decode has it.  Every thread calls it, right after a barrier.
+        auto try_switch = [&]() {
+            if (!may_switch || !sym || out < mark_end + WV_WINDOW) return;
+            const uint64_t area = (2 * out + 15) & ~(uint64_t)15;   // byte offset in job.dst of the window's copy
+            const uint64_t room = 2 * job.dst_cap;                   // bytes of job.dst (the store slack lies behind)
+            if (area + WV_WINDOW > room) return;                     // no room: stay symbolic
+            const uint16_t* const s16 = reinterpret_cast<const uint16_t*>(job.dst);
+            uint8_t* const        nd  = job.dst + area + WV_WINDOW - out;   // nd[x] = byte x, x >= out - 32768
+            for (uint64_t x = out - WV_WINDOW + t; x < out; x += WV_THREADS) nd[x] = (uint8_t)s16[x];
+            __syncthreads();
+            sym        = false;
+            esz        = 1;
+            dst        = nd;
+            dst_cap    = room - area - WV_WINDOW + out;
+            mis        = (uint32_t)((uintptr_t)nd & 15);
+            ring_stale = true;
+            sw_out     = out;
+            sw_bytes   = area + WV_WINDOW;
         };
 
         if (phase == 0) {
@@ -799,7 +828,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
             tick(0);
             if (type == 0) {
                 if (!br.have(8 * (uint64_t)stored)) { st = PNGB200_NEED_MORE_INPUT; break; }
-                if (out + stored > job.dst_cap) { st = fail(r, PNGB200_ERR_OUTPUT_CAPACITY); break; }
+                if (out + stored > dst_cap) { st = fail(r, PNGB200_ERR_OUTPUT_CAPACITY); break; }
                 const uint8_t* s = job.src + (br.at() >> 3);
                 if (sym) for (uint32_t k = t; k < stored; k += WV_THREADS) reinterpret_cast<uint16_t*>(dst)[out + k] = s[k];
                 else for (uint32_t k = t; k < stored; k += WV_THREADS) dst[out + k] = s[k];
@@ -809,6 +838,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                 br.seek(br.pos + 8 * (uint64_t)stored);
                 __syncthreads();
                 fold_adler();
+                try_switch();
                 tick(9);
             } else {
                 bool block_done = false;
@@ -1080,8 +1110,9 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                     const uint32_t c_start = (uint32_t)(excl >> 40);           // my first list slot
                     const uint64_t total64 = sh.warp_sums[WV_WARPS] & 0xffffffffffull;
                     const uint32_t np      = (uint32_t)(sh.warp_sums[WV_WARPS] >> 40);
-                    if (sh.anomaly || out + total64 > job.dst_cap || total64 > P.bitmap_words * 32) {
+                    if (sh.anomaly || out + total64 > dst_cap || total64 > P.bitmap_words * 32) {
                         fallback = true;
+                        over_cap = out + total64 > dst_cap;
                         break;
                     }
                     const uint32_t  total  = (uint32_t)total64;
@@ -1231,6 +1262,20 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                         fallback = true;
                         break;
                     }
+                    if (may_switch && sym) {
+                        // the wave's last marker, read back from L2 (only while the tail is still symbolic)
+                        const uint16_t* const ws = reinterpret_cast<const uint16_t*>(wdst);
+                        uint32_t lm = 0;
+                        for (uint32_t k = t; k < total; k += WV_THREADS)
+                            if (ws[k] & 0x8000u) lm = k + 1;
+                        for (int o = 16; o; o >>= 1) lm = max(lm, __shfl_xor_sync(0xffffffffu, lm, o));
+                        if (lane == 0) sh.mark[warp] = lm;
+                        __syncthreads();
+                        uint32_t wm = 0;
+#pragma unroll
+                        for (int w = 0; w < WV_WARPS; ++w) wm = max(wm, sh.mark[w]);
+                        if (wm) mark_end = out + wm;
+                    }
                     // ---- G. store: ring -> HBM, 16-byte coalesced; Adler-32 partial sums from the same registers ----
                     if (!in_hbm && total) {
                         const uint32_t shift = rbase & 15u;                  // == (uintptr_t)wdst & 15
@@ -1274,6 +1319,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                     n_deferred += deferred;
                     br.seek((wbase << 5) + sh.wpos_[last]);
                     if (term == WK_EOB || term == WK_OWN_EOB) block_done = true;
+                    try_switch();
                 }
                 if (fallback) break;
             }
@@ -1330,10 +1376,11 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                 for (int k = 0; k < 12; ++k) r->stat_cycles[k] = sh.cyc[k];
             }
         }
-        if (fallback && sym) {
+        if (fallback && job.symbolic) {
             // a segment cannot go through the byte-wise serial decoder: report it, the host decodes the stream whole
+            // (a tail whose bytes ran out of room behind its symbols says so)
             if (t == 0) {
-                r->status = PNGB200_ERR_INTERNAL;
+                r->status = sw_out != ~0ull && over_cap ? PNGB200_ERR_OUTPUT_CAPACITY : PNGB200_ERR_INTERNAL;
                 r->produced = out;
                 r->consumed_bits = br.at();
                 r->blocks = blocks;
@@ -1363,6 +1410,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
             }
         }
         if (t == 0) r->stat_fallback = fallback ? 1u : 0u;
+        if (t == 0 && may_switch && P.switched) P.switched[j] = SwitchRecord{sw_out != ~0ull ? sw_out : out, sw_bytes};
     }
 }
 

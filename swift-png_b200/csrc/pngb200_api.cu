@@ -111,6 +111,7 @@ struct pngb200_ctx {
     // pinned host tables
     PinBuf h_jobs, h_results, h_imgjobs, h_genjobs, h_misc, h_order, h_crc, h_seg, h_sgsearch, h_sgjobs, h_sgres, h_sgrec;
     uint64_t seg_streams = 0, seg_segments = 0, seg_fallbacks = 0;  // last batch: streams cut into segments, segments, rejected
+    uint64_t split_stats[6] = {};      // last batch, streams cut in two: see pngb200_ctx_split_stats
     uint64_t scratch_stride = 0;       // layout of d_scratch the last inflate launch used
     size_t parallel_threshold = 8192;  // streams at least this long use the block-parallel kernel
     unsigned long long* d_hist = nullptr;   // filter-type histogram of the last wavefront-unfilter launch (in d_imgjobs)
@@ -380,18 +381,23 @@ int run_segments(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t
 size_t plan_slots(const pngb200_ctx* ctx) { return ctx->plan_slots ? ctx->plan_slots : (size_t)ctx->sm_count * WV_CTAS_PER_SM; }
 
 // ---- a stream cut in two: a direct head and a symbolic tail (inflate_segments.cuh, DESIGN.md section 4.2) ----
-// Per output byte, inflate_wave_kernel in symbolic mode (tails) costs this many times what it costs writing bytes
-// (heads): stat_cycles over produced, 13.8 against 10.0 cycles per byte, for the 198 x 7680x4320 RGBA8 photo batch
-// (bench.py's default) cut at h = 0.78, on an H100 80GB HBM3 at a 400 W power limit and 1980 MHz.
-constexpr double kSymbolicCost = 1.38;
+// Per output byte, a tail costs this many times what a head costs: stat_cycles over produced (tools/split_cost.py),
+// 10.64 against 10.12 cycles per byte, for the 198 x 7680x4320 RGBA8 photo batch (bench.py's default) cut at
+// h = 0.763, on an H100 80GB HBM3 at a 700 W power limit and 1980 MHz.  A tail decodes symbols (about 1.38x a head's
+// cost per byte) only until its last 32 KiB hold no marker, 10.3 % of its bytes on that batch, and bytes like a head
+// after that.
+constexpr double kSymbolicCost = 1.05;
 
 // B big streams on N CTA slots with N / 2 < B < N: one CTA per stream would leave N - B slots idle for the whole
 // launch.  Each stream is cut at a block boundary instead: heads take the first B tickets, the N - B other CTAs
 // work through the tails one after another.  Head share h = B rho / (N - B + B rho) gives a chain of B / (N - B)
 // tails the cost of one head.  The tail's symbols go to the stream's scratch (the image's pixel buffer, dead until
-// unfilter); the head's bytes are final where they land.  On return `par` holds the streams still to be decoded
-// whole: not cut, or cut but not accepted (split_finish_kernel) -- so statuses and errors are those of the
-// whole-stream path for every input.
+// unfilter), and once the tail leaves symbolic mode its bytes go behind them (StreamJob.may_switch): 2m + 32 KiB +
+// (n2 - m) bytes for a tail of n2 bytes that switched at m, at most the 2 n2 of a tail that never does, which is what
+// the scratch guard below provides for (with a margin for tails longer than 1 - h of the stream); a switched tail
+// that still runs out of room fails and its stream is decoded whole.  The head's bytes are final where they land.
+// On return `par` holds the streams still to be decoded whole: not cut, or cut but not accepted (split_finish_kernel)
+// -- so statuses and errors are those of the whole-stream path for every input.
 
 // the head share h when the big streams `par` are to be cut, else 0
 double split_head_share(const pngb200_ctx* ctx, const StreamJob* h_jobs, const std::vector<uint32_t>& par)
@@ -433,7 +439,10 @@ int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& 
     if (n == 0) return PNGB200_OK;
     CU(ctx->h_sgjobs.reserve(sizeof(StreamJob) * 2 * n));
     CU(ctx->d_sgjobs.reserve(sizeof(StreamJob) * 2 * n));
-    CU(ctx->d_sgres.reserve(sizeof(StreamResult) * 2 * n));
+    // the pieces' results, then where each job left symbolic mode (SwitchRecord; only the tails' are written)
+    const size_t res_bytes = sizeof(StreamResult) * 2 * n + sizeof(SwitchRecord) * 2 * n;
+    static_assert(sizeof(StreamResult) % alignof(SwitchRecord) == 0, "switch records behind the results");
+    CU(ctx->d_sgres.reserve(res_bytes));
     StreamJob* sg = ctx->h_sgjobs.as<StreamJob>();
     uint64_t max_cap = 0;
     for (size_t k = 0, s = 0; k < nb; ++k) {
@@ -448,12 +457,14 @@ int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& 
         tl.start_bit = sj[k].found;
         tl.phase = 1;
         tl.symbolic = 1;
+        tl.may_switch = 1;
         tl.dst = j.scratch;
         tl.dst_cap = j.scratch_cap / 2 - 64;   // symbols, with the kernel's store slack behind them
         max_cap = std::max(max_cap, j.dst_cap);
     }
     CU(cudaMemcpyAsync(ctx->d_sgjobs.p, sg, sizeof(StreamJob) * 2 * n, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemsetAsync(ctx->d_sgres.p, 0, sizeof(StreamResult) * 2 * n, ctx->stream));
+    CU(cudaMemsetAsync(ctx->d_sgres.p, 0, res_bytes, ctx->stream));
+    SwitchRecord* d_switch = (SwitchRecord*)(ctx->d_sgres.as<StreamResult>() + 2 * n);
     {
         WvParams pp;
         pp.bitmap_words = wv_bitmap_words(max_cap);
@@ -472,6 +483,7 @@ int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& 
         pp.order = nullptr;
         pp.scratch = ctx->d_scratch.as<uint8_t>();
         pp.count = (int)(2 * n);
+        pp.switched = d_switch;
         inflate_wave_kernel<<<grid, WV_THREADS, sizeof(WvShared), ctx->stream>>>(pp);
         ctx->launches++;
     }
@@ -486,7 +498,7 @@ int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& 
     for (size_t s = 0; s < n; ++s) {
         const StreamJob& j = h_jobs[cut[s]];
         rec[s] = SplitRecord{d_sgres + s, d_sgres + n + s, (const uint16_t*)j.scratch, j.dst, j.dst_cap, sg[s].stop_bit,
-                             ctx->d_results.as<StreamResult>() + cut[s]};
+                             ctx->d_results.as<StreamResult>() + cut[s], d_switch + n + s};
     }
     CU(cudaMemcpyAsync(ctx->d_sgrec.p, rec, sizeof(SplitRecord) * n, cudaMemcpyHostToDevice, ctx->stream));
     const SplitRecord* d_rec = ctx->d_sgrec.as<SplitRecord>();
@@ -498,14 +510,30 @@ int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& 
     CU(cudaGetLastError());
     uint32_t* accept = (uint32_t*)((char*)ctx->h_sgrec.p + off_accept);
     CU(cudaMemcpyAsync(accept, d_accept, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(ctx->h_sgres.reserve(res_bytes));
+    CU(cudaMemcpyAsync(ctx->h_sgres.p, d_sgres, res_bytes, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     ctx->seg_streams += n;
     ctx->seg_segments += 2 * n;
-    for (size_t s = 0; s < n; ++s)
+    const StreamResult* pieces = ctx->h_sgres.as<StreamResult>();
+    const SwitchRecord* switched = (const SwitchRecord*)(pieces + 2 * n);
+    for (size_t s = 0; s < n; ++s) {
         if (!accept[s]) {
             ctx->seg_fallbacks++;
             rest.push_back(cut[s]);
+            continue;
         }
+        const StreamResult &hd = pieces[s], &tl = pieces[n + s];
+        ctx->split_stats[0] += hd.produced;
+        ctx->split_stats[2] += tl.produced;
+        for (int q = 0; q < 12; ++q) {
+            ctx->split_stats[1] += hd.stat_cycles[q];
+            ctx->split_stats[3] += tl.stat_cycles[q];
+        }
+        const SwitchRecord& sw = switched[n + s];
+        ctx->split_stats[4] += sw.out < tl.produced;
+        ctx->split_stats[5] += sw.out;
+    }
     // what is left keeps its longest-first order
     std::vector<uint32_t> left;
     for (uint32_t i : par)
@@ -522,6 +550,7 @@ int run_inflate(pngb200_ctx* ctx, const StreamJob* h_jobs, size_t count)
     StreamJob*    d_jobs    = ctx->d_jobs.as<StreamJob>();
     StreamResult* d_results = ctx->d_results.as<StreamResult>();
     ctx->seg_streams = ctx->seg_segments = ctx->seg_fallbacks = 0;
+    for (uint64_t& v : ctx->split_stats) v = 0;
     CU(cudaMemsetAsync(d_results, 0, sizeof(StreamResult) * count, ctx->stream));
     auto before_first_launch = [&]() -> int {
         int rc = PNGB200_OK;
@@ -1115,6 +1144,13 @@ int pngb200_ctx_filter_histogram(pngb200_ctx* ctx, uint64_t out[6])
 
 int pngb200_ctx_last_inflate_engine(pngb200_ctx* ctx) { return ctx ? ctx->last_engine : -1; }
 
+int pngb200_ctx_split_stats(pngb200_ctx* ctx, uint64_t out[6])
+{
+    if (!ctx || !out) return PNGB200_ERR_BAD_ARGUMENT;
+    for (int k = 0; k < 6; ++k) out[k] = ctx->split_stats[k];
+    return PNGB200_OK;
+}
+
 int pngb200_ctx_segment_stats(pngb200_ctx* ctx, uint64_t out[3])
 {
     if (!ctx || !out) return PNGB200_ERR_BAD_ARGUMENT;
@@ -1178,7 +1214,7 @@ int pngb200_inflate_batch(pngb200_ctx* ctx, pngb200_stream_desc* s, size_t count
         jobs[i].phase = 0;
         jobs[i].stop_bit = 0;
         jobs[i].symbolic = 0;
-        jobs[i].pad_ = 0;
+        jobs[i].may_switch = 0;
         jobs[i].scratch = nullptr;   // no buffer to borrow: streams are not cut in two
         jobs[i].scratch_cap = 0;
     }
@@ -1263,7 +1299,7 @@ int pngb200_decode_batch_enqueue(pngb200_ctx* ctx, pngb200_image_desc* im, size_
         jobs[i].phase = 0;
         jobs[i].stop_bit = 0;
         jobs[i].symbolic = 0;
-        jobs[i].pad_ = 0;
+        jobs[i].may_switch = 0;
         // the pixel buffer is dead until unfilter writes it: a stream cut in two keeps its tail's symbols there
         // (host batches run lanes side by side and are not cut)
         jobs[i].scratch = host ? nullptr : im[i].pixels;
@@ -1907,7 +1943,7 @@ int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
         job->phase = (int32_t)z->phase;
         job->stop_bit = 0;
         job->symbolic = 0;
-        job->pad_ = 0;
+        job->may_switch = 0;
         CU(cudaMemcpyAsync(z->d_job.p, job, sizeof(StreamJob), cudaMemcpyHostToDevice, ctx->stream));
         CU(cudaMemsetAsync(z->d_res.p, 0, sizeof(StreamResult), ctx->stream));
         // A push with a lot of undecoded input goes through the intra-stream parallel kernel (one CTA: ~25 x the

@@ -142,6 +142,25 @@ static int decode_segment(const uint8_t* in, size_t n, uint64_t start, const uin
     }
 }
 
+/* The tail of a stream cut in two (DESIGN.md section 4.2): decoded from the block header at `start` to the end of
+ * the stream with the 32 KiB in front unknown.  out[0] output bytes; out[1] the first output offset whose last
+ * 32 KiB hold no marker (from there on nothing can depend on the head; out[0] if the tail never gets there);
+ * out[2] markers.  Returns 0, or -1 when the decode fails (`start` is not a real block boundary). */
+int tail_model(const uint8_t* in, size_t n, uint64_t start, uint64_t* out)
+{
+    symbuf   s = {0};
+    uint64_t end, last = 0, markers = 0;   /* last: 1 + offset of the last marker */
+    const int rc = decode_segment(in, n, start, NULL, 0, 0, &s, &end);
+    if (rc >= 0)
+        for (size_t i = 0; i < s.n; ++i)
+            if (s.sym[i] >= 256) { last = i + 1; ++markers; }
+    out[0] = s.n;
+    out[1] = last + 32768 < s.n ? last + 32768 : s.n;
+    out[2] = markers;
+    free(s.sym);
+    return rc >= 0 ? 0 : -1;
+}
+
 /* Whole model.  stats[4 * k + ...] per accepted segment: start bit, symbols, markers, markers beyond
  * the first 32 KiB.  Returns output length (0 on failure); *nsegments = segments actually joined. */
 size_t segment_model(const uint8_t* in, size_t n, int want, uint8_t* out, size_t cap, uint64_t* stats, int* nsegments,
