@@ -381,11 +381,7 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                 if (warp == 0) {
                     WvHeader h;
                     uint32_t rel = 0;
-#ifdef CL_SERIAL_HEADER   // (tuning builds: the code lengths by one lane, as in inflate_wave_kernel)
-                    const int mode = wv_fast_header(sh, hbase << 5, br.pos, br.total_bits, (int)lane, h) ? 1 : 0;
-#else
                     const int mode = cl_header_preamble(sh, hbase << 5, br.pos, br.total_bits, (int)lane, h, rel);
-#endif
                     if (mode == 0) slow_header(h);
                     if (lane == 0) {
                         sh.hdr = h;
@@ -791,9 +787,6 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                     const uint32_t reach = (sym || out >= WV_WINDOW) ? 0x7fffffffu : (uint32_t)out;
                     uint32_t emitted = 0, my_stop = 0xffffffffu, o = 0;
                     [[maybe_unused]] uint32_t from_staging = 0;   // (cost-model counter of emulator builds)
-#ifdef CL_NO_STAGING
-                    kept = false;
-#endif
                     if ((on_chain || adopted) && from != to && !cut && kept) {
                         // my share was kept by the passes that decoded it: read it back (walk piece, own piece, own walk)
                         o = (uint32_t)o64;

@@ -53,9 +53,6 @@ constexpr int      PAR_WARPS        = PAR_THREADS / 32;
 #ifndef PAR_S
 #define PAR_S 256
 #endif
-#ifndef PAR_NO_OPAQUE_BASE
-#define PAR_OPAQUE_BASE 1   // decode loops address shared memory from a base the compiler cannot rebuild from SR_CgaCtaId
-#endif
 constexpr uint32_t PAR_SUB_BITS     = PAR_S;
 constexpr uint32_t PAR_SUB_WORDS    = PAR_SUB_BITS / 32;
 constexpr uint32_t PAR_WAVE_WORDS   = PAR_THREADS * PAR_SUB_WORDS + 8;
@@ -111,14 +108,10 @@ __device__ __forceinline__ void par_decode_count(const ParShared& sh, uint32_t s
                                                  uint32_t& flags)
 {
     FastBits b;
-#ifdef PAR_OPAQUE_BASE
+    // shared memory addressed from a base the compiler cannot rebuild from SR_CgaCtaId inside the loop
     const saddr_t sb = opaque(smem_addr(&sh));
     b.init(sb + offsetof(ParShared, words), start);
     const saddr_t lit = sb + offsetof(ParShared, ser) + offsetof(SerialShared, lit), dst = sb + offsetof(ParShared, ser) + offsetof(SerialShared, dist);
-#else
-    b.init(smem_addr(sh.words), start);
-    const saddr_t lit = smem_addr(sh.ser.lit), dst = smem_addr(sh.ser.dist);
-#endif
     nout  = 0;
     ncopy = 0;
     flags = 0;
@@ -472,14 +465,9 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
                     uint32_t* const U      = in_hbm ? gbitmap : sh.bitmap;
                     if (t < nvalid) {
                         FastBits b;
-#ifdef PAR_OPAQUE_BASE
-                        const saddr_t sb = opaque(smem_addr(&sh));
+                        const saddr_t sb = opaque(smem_addr(&sh));   // (see par_decode_count)
                         b.init(sb + offsetof(ParShared, words), my_start);
                         const saddr_t lit = sb + offsetof(ParShared, ser) + offsetof(SerialShared, lit), dst = sb + offsetof(ParShared, ser) + offsetof(SerialShared, dist);
-#else
-                        b.init(smem_addr(sh.words), my_start);
-                        const saddr_t lit = smem_addr(sh.ser.lit), dst = smem_addr(sh.ser.dist);
-#endif
                         uint32_t o = o_start;
                         uint32_t mw = o_start >> 5, mbits = 0;   // pending unresolved-bit word
                         while (b.pos < limit) {

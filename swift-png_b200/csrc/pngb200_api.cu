@@ -97,9 +97,6 @@ struct pngb200_ctx {
     uint64_t     launches = 0;
     int          inflate_mode = 0;
     int          last_engine = -1;       // whole-stream engine of the last batch: 0 round-1, 1 ring, 2 cells, -1 none
-    bool         cells_auto = false;     // automatic mode may pick inflate_cells_kernel (set once measured faster)
-    bool         cells_segments = true;  // segments (several CTAs per stream) are decoded by inflate_cells_kernel: 3 CTA slots per SM instead
-                                         // of 2 (PNGB200_CELLS_SEGMENTS=0 restores the ring kernel)
     int          sm_count = 132;
     size_t       device_bytes = 0;     // global memory of the device (sizes the deflate scratch arena)
     std::string  error;
@@ -181,6 +178,85 @@ int ensure_crc_tables(pngb200_ctx* ctx)
     return PNGB200_OK;
 }
 
+// a job that decodes a whole stream from its header into dst
+StreamJob whole_stream_job(const uint8_t* src, uint64_t src_len, uint8_t* dst, uint64_t dst_cap, int32_t format)
+{
+    StreamJob j{};
+    j.src = src;
+    j.src_len = src_len;
+    j.dst = dst;
+    j.dst_cap = dst_cap;
+    j.format = format;
+    return j;
+}
+
+// The engines that decode big streams in waves of 256 subsequences, numbered as pngb200_ctx_last_inflate_engine reports them
+enum Engine { ENG_PARALLEL = 0, ENG_WAVE = 1, ENG_CELLS = 2 };
+
+// One launch of a wave engine: `grid` persistent CTAs pull the `count` jobs from a ticket, through `order` when it is
+// not null.  `max_cap`: the largest dst_cap the per-CTA HBM bitmaps have to cover (the cell engine has none).
+// `switched`: a SwitchRecord per job, for jobs with may_switch (ring engine), or null.  `before_launch`, when given,
+// is enqueued after the scratch set-up and right before the kernel.
+int launch_waves(pngb200_ctx* ctx, Engine engine, const StreamJob* jobs, StreamResult* results, const uint32_t* order, size_t count,
+                 unsigned grid, uint64_t max_cap, SwitchRecord* switched, const std::function<int()>& before_launch = nullptr)
+{
+    const uint64_t bitmap_words = engine == ENG_WAVE ? wv_bitmap_words(max_cap) : engine == ENG_PARALLEL ? par_bitmap_words(max_cap) : 0;
+    const uint64_t stride = engine == ENG_WAVE       ? wv_scratch_stride(bitmap_words)
+                            : engine == ENG_PARALLEL ? par_scratch_stride(bitmap_words)
+                                                     : CL_SCRATCH;
+    // d_scratch holds `stride` bytes per CTA, then the ticket.  The per-CTA "unresolved" bitmaps must be all-zero when
+    // a launch starts; the kernels leave them clean.  A different stride moves the bitmaps onto bytes that held copy
+    // lists before, and a fresh allocation is garbage: zero the whole arena in both cases.
+    const size_t need = (size_t)stride * grid + 256;
+    if (need > ctx->d_scratch.cap || stride != ctx->scratch_stride) {
+        CU(ctx->d_scratch.reserve(need));
+        CU(cudaMemsetAsync(ctx->d_scratch.p, 0, ctx->d_scratch.cap, ctx->stream));
+        ctx->scratch_stride = stride;
+    }
+    uint32_t* ticket = (uint32_t*)((char*)ctx->d_scratch.p + (size_t)stride * grid);
+    CU(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), ctx->stream));
+    if (before_launch)
+        if (int rc = before_launch()) return rc;
+    auto fill = [&](auto& pp) {
+        pp.jobs = jobs;
+        pp.results = results;
+        pp.order = order;
+        pp.ticket = ticket;
+        pp.scratch = ctx->d_scratch.as<uint8_t>();
+        pp.scratch_stride = stride;
+        pp.bitmap_words = bitmap_words;
+        pp.count = (int)count;
+    };
+    if (engine == ENG_PARALLEL) {
+        ParParams pp{};
+        fill(pp);
+        if (count <= (size_t)ctx->sm_count * 3)
+            inflate_parallel_kernel3<<<grid, PAR_THREADS, sizeof(ParShared), ctx->stream>>>(pp);
+        else
+            inflate_parallel_kernel<<<grid, PAR_THREADS, sizeof(ParShared), ctx->stream>>>(pp);
+    } else {
+        WvParams pp{};
+        fill(pp);
+        pp.switched = switched;
+        if (engine == ENG_CELLS) inflate_cells_kernel<<<grid, WV_THREADS, sizeof(ClShared), ctx->stream>>>(pp);
+        else inflate_wave_kernel<<<grid, WV_THREADS, sizeof(WvShared), ctx->stream>>>(pp);
+    }
+    ctx->launches++;
+    return PNGB200_OK;
+}
+
+// the first plausible dynamic-block header of each of the n SearchJobs in h_sgsearch (found, or ~0), one host round trip
+int search_blocks(pngb200_ctx* ctx, size_t n)
+{
+    CU(ctx->d_sgsearch.reserve(sizeof(SearchJob) * n));
+    CU(cudaMemcpyAsync(ctx->d_sgsearch.p, ctx->h_sgsearch.p, sizeof(SearchJob) * n, cudaMemcpyHostToDevice, ctx->stream));
+    block_search_kernel<<<dim3((unsigned)n, BS_CTAS), 256, 0, ctx->stream>>>(ctx->d_sgsearch.as<SearchJob>(), (uint32_t)n);
+    ctx->launches++;
+    CU(cudaMemcpyAsync(ctx->h_sgsearch.p, ctx->d_sgsearch.p, sizeof(SearchJob) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    return PNGB200_OK;
+}
+
 // ---- more than one CTA per stream (inflate_segments.cuh) ----
 // Streams of `par` that are worth cutting are decoded here, segment by segment; on return `par` holds the
 // streams that still have to go through the whole-stream kernels (not cut, or a segment did not line up).
@@ -189,7 +265,7 @@ int ensure_crc_tables(pngb200_ctx* ctx)
 int run_segments(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& par)
 {
     ctx->seg_streams = ctx->seg_segments = ctx->seg_fallbacks = 0;
-    const size_t slots = (size_t)ctx->sm_count * (ctx->cells_segments ? CL_CTAS_PER_SM : WV_CTAS_PER_SM);
+    const size_t slots = (size_t)ctx->sm_count * CL_CTAS_PER_SM;
     constexpr uint64_t kMinSegment = 256u << 10;  // compressed bytes per segment, at least
     if (par.empty() || par.size() * 2 > slots) return PNGB200_OK;
     const size_t per_stream = std::max<size_t>(1, slots / par.size());
@@ -205,7 +281,6 @@ int run_segments(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t
     if (cuts.empty()) return PNGB200_OK;
     // 1. split points: the first plausible dynamic-block header at or after k / nseg of the stream
     CU(ctx->h_sgsearch.reserve(sizeof(SearchJob) * nsearch));
-    CU(ctx->d_sgsearch.reserve(sizeof(SearchJob) * nsearch));
     SearchJob* sj = ctx->h_sgsearch.as<SearchJob>();
     for (const Cut& c : cuts) {
         const StreamJob& j = h_jobs[c.stream];
@@ -219,16 +294,11 @@ int run_segments(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t
             q.found = ~0ull;
         }
     }
-    CU(cudaMemcpyAsync(ctx->d_sgsearch.p, sj, sizeof(SearchJob) * nsearch, cudaMemcpyHostToDevice, ctx->stream));
-    block_search_kernel<<<dim3((unsigned)nsearch, BS_CTAS), 256, 0, ctx->stream>>>(ctx->d_sgsearch.as<SearchJob>(), (uint32_t)nsearch);
-    ctx->launches++;
-    CU(cudaMemcpyAsync(sj, ctx->d_sgsearch.p, sizeof(SearchJob) * nsearch, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
+    if (int rc = search_blocks(ctx, nsearch)) return rc;
     // 2. one job per segment; symbols go to a scratch sized 1.5 x the segment's share of the output bound
     std::vector<StreamJob> sg;
     std::vector<uint32_t>  sg_stream, first_of;   // stream of each segment; first segment of each cut (+ end)
     size_t sym_total = 0;
-    uint64_t max_cap = 0;
     for (const Cut& c : cuts) {
         const StreamJob& j = h_jobs[c.stream];
         std::vector<uint64_t> at{0};
@@ -246,7 +316,6 @@ int run_segments(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t
             s.dst_cap = (uint64_t)((double)j.dst_cap * 1.5 * (double)(end - at[k]) / (double)(8 * j.src_len)) + (64u << 10);
             s.dst = (uint8_t*)(uintptr_t)sym_total;  // offset for now (symbols)
             sym_total += align_up(s.dst_cap + 8, 128);
-            max_cap = std::max(max_cap, s.dst_cap);
             sg.push_back(s);
             sg_stream.push_back(c.stream);
         }
@@ -262,28 +331,9 @@ int run_segments(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t
     memcpy(ctx->h_sgjobs.p, sg.data(), sizeof(StreamJob) * n);
     CU(cudaMemcpyAsync(ctx->d_sgjobs.p, ctx->h_sgjobs.p, sizeof(StreamJob) * n, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_sgres.p, 0, sizeof(StreamResult) * n, ctx->stream));
-    {
-        WvParams pp;
-        pp.bitmap_words = ctx->cells_segments ? 8 : wv_bitmap_words(max_cap);
-        pp.scratch_stride = ctx->cells_segments ? CL_SCRATCH : wv_scratch_stride(pp.bitmap_words);
-        unsigned grid = (unsigned)std::min<size_t>(n, slots);
-        size_t need = (size_t)pp.scratch_stride * grid + 256;
-        if (need > ctx->d_scratch.cap || pp.scratch_stride != ctx->scratch_stride) {
-            CU(ctx->d_scratch.reserve(need));
-            CU(cudaMemsetAsync(ctx->d_scratch.p, 0, ctx->d_scratch.cap, ctx->stream));
-            ctx->scratch_stride = pp.scratch_stride;
-        }
-        pp.ticket = (uint32_t*)((char*)ctx->d_scratch.p + (size_t)pp.scratch_stride * grid);
-        CU(cudaMemsetAsync(pp.ticket, 0, sizeof(uint32_t), ctx->stream));
-        pp.jobs = ctx->d_sgjobs.as<StreamJob>();
-        pp.results = ctx->d_sgres.as<StreamResult>();
-        pp.order = nullptr;
-        pp.scratch = ctx->d_scratch.as<uint8_t>();
-        pp.count = (int)n;
-        if (ctx->cells_segments) inflate_cells_kernel<<<grid, WV_THREADS, sizeof(ClShared), ctx->stream>>>(pp);
-        else inflate_wave_kernel<<<grid, WV_THREADS, sizeof(WvShared), ctx->stream>>>(pp);
-        ctx->launches++;
-    }
+    if (int rc = launch_waves(ctx, ENG_CELLS, ctx->d_sgjobs.as<StreamJob>(), ctx->d_sgres.as<StreamResult>(), nullptr, n,
+                              (unsigned)std::min<size_t>(n, slots), 0, nullptr))
+        return rc;
     CU(cudaMemcpyAsync(ctx->h_sgres.p, ctx->d_sgres.p, sizeof(StreamResult) * n, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     // 3. a stream is accepted when every segment ended exactly where the next one starts
@@ -421,17 +471,12 @@ int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& 
     const size_t slots = plan_slots(ctx), nb = par.size();
     // 1. split points: the first plausible dynamic-block header at or after h of the stream
     CU(ctx->h_sgsearch.reserve(sizeof(SearchJob) * nb));
-    CU(ctx->d_sgsearch.reserve(sizeof(SearchJob) * nb));
     SearchJob* sj = ctx->h_sgsearch.as<SearchJob>();
     for (size_t k = 0; k < nb; ++k) {
         const StreamJob& j = h_jobs[par[k]];
         sj[k] = SearchJob{j.src, j.src_len, (uint64_t)(h * (double)(8 * j.src_len)), 8 * j.src_len, ~0ull};
     }
-    CU(cudaMemcpyAsync(ctx->d_sgsearch.p, sj, sizeof(SearchJob) * nb, cudaMemcpyHostToDevice, ctx->stream));
-    block_search_kernel<<<dim3((unsigned)nb, BS_CTAS), 256, 0, ctx->stream>>>(ctx->d_sgsearch.as<SearchJob>(), (uint32_t)nb);
-    ctx->launches++;
-    CU(cudaMemcpyAsync(sj, ctx->d_sgsearch.p, sizeof(SearchJob) * nb, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaStreamSynchronize(ctx->stream));
+    if (int rc = search_blocks(ctx, nb)) return rc;
     // 2. heads (LPT order, first tickets), then the tails in the same order
     std::vector<uint32_t> cut, rest;
     for (size_t k = 0; k < nb; ++k) (sj[k].found != ~0ull ? cut : rest).push_back(par[k]);
@@ -465,28 +510,9 @@ int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& 
     CU(cudaMemcpyAsync(ctx->d_sgjobs.p, sg, sizeof(StreamJob) * 2 * n, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_sgres.p, 0, res_bytes, ctx->stream));
     SwitchRecord* d_switch = (SwitchRecord*)(ctx->d_sgres.as<StreamResult>() + 2 * n);
-    {
-        WvParams pp;
-        pp.bitmap_words = wv_bitmap_words(max_cap);
-        pp.scratch_stride = wv_scratch_stride(pp.bitmap_words);
-        const unsigned grid = (unsigned)std::min<size_t>(2 * n, slots);
-        const size_t need = (size_t)pp.scratch_stride * grid + 256;
-        if (need > ctx->d_scratch.cap || pp.scratch_stride != ctx->scratch_stride) {   // bitmaps start zeroed (see run_inflate)
-            CU(ctx->d_scratch.reserve(need));
-            CU(cudaMemsetAsync(ctx->d_scratch.p, 0, ctx->d_scratch.cap, ctx->stream));
-            ctx->scratch_stride = pp.scratch_stride;
-        }
-        pp.ticket = (uint32_t*)((char*)ctx->d_scratch.p + (size_t)pp.scratch_stride * grid);
-        CU(cudaMemsetAsync(pp.ticket, 0, sizeof(uint32_t), ctx->stream));
-        pp.jobs = ctx->d_sgjobs.as<StreamJob>();
-        pp.results = ctx->d_sgres.as<StreamResult>();
-        pp.order = nullptr;
-        pp.scratch = ctx->d_scratch.as<uint8_t>();
-        pp.count = (int)(2 * n);
-        pp.switched = d_switch;
-        inflate_wave_kernel<<<grid, WV_THREADS, sizeof(WvShared), ctx->stream>>>(pp);
-        ctx->launches++;
-    }
+    if (int rc = launch_waves(ctx, ENG_WAVE, ctx->d_sgjobs.as<StreamJob>(), ctx->d_sgres.as<StreamResult>(), nullptr, 2 * n,
+                              (unsigned)std::min<size_t>(2 * n, slots), max_cap, d_switch))
+        return rc;
     // 3. tails -> bytes behind their heads, Adler-32 of the whole stream, acceptance; device-side, one host round trip
     const size_t off_accept  = align_up(sizeof(SplitRecord) * n, 256);
     const size_t off_partial = align_up(off_accept + sizeof(uint32_t) * n, 256);
@@ -552,7 +578,10 @@ int run_inflate(pngb200_ctx* ctx, const StreamJob* h_jobs, size_t count)
     ctx->seg_streams = ctx->seg_segments = ctx->seg_fallbacks = 0;
     for (uint64_t& v : ctx->split_stats) v = 0;
     CU(cudaMemsetAsync(d_results, 0, sizeof(StreamResult) * count, ctx->stream));
-    auto before_first_launch = [&]() -> int {
+    bool hooked = false;
+    auto before_first_launch = [&]() -> int {   // once, in front of the batch's first kernel
+        if (hooked) return PNGB200_OK;
+        hooked = true;
         int rc = PNGB200_OK;
         if (ctx->bulk_h2d) {
             rc = ctx->bulk_h2d();
@@ -580,17 +609,14 @@ int run_inflate(pngb200_ctx* ctx, const StreamJob* h_jobs, size_t count)
         std::copy(ser.begin(), ser.end(), ho + par.size());
         CU(cudaMemcpyAsync(ctx->d_order.p, ho, sizeof(uint32_t) * count, cudaMemcpyHostToDevice, ctx->stream));
         const uint32_t* d_order = ctx->d_order.as<uint32_t>();
-        bool hooked = false;
         if (ctx->inflate_mode == 0 || ctx->inflate_mode == 5) {
             // few big streams: cut them so that every CTA slot has something to decode
             const size_t before = par.size();
             if (!par.empty() && std::max(par.size(), ctx->peer_streams) * 2 <= plan_slots(ctx)) {
                 if (int rc = before_first_launch()) return rc;
-                hooked = true;
                 if (int rc = run_segments(ctx, h_jobs, par)) return rc;
             } else if (const double h = split_head_share(ctx, h_jobs, par)) {
                 if (int rc = before_first_launch()) return rc;
-                hooked = true;
                 if (int rc = run_split(ctx, h_jobs, par, h)) return rc;
             }
             if (par.size() != before) {   // the order table lists what is left for the whole-stream kernels
@@ -602,91 +628,32 @@ int run_inflate(pngb200_ctx* ctx, const StreamJob* h_jobs, size_t count)
         if (!par.empty()) {
             uint64_t max_cap = 0;
             for (uint32_t i : par) max_cap = std::max<uint64_t>(max_cap, h_jobs[i].dst_cap);
-            // Two engines for the big streams, same decomposition (8 KiB waves of 256 subsequences), chosen by
-            // how many streams there are to keep the SMs busy:
+            // Three engines for the big streams, same decomposition (8 KiB waves of 256 subsequences):
             //  * inflate_wave_kernel: LZ77 window in a 64 KiB shared-memory ring, Adler-32 folded into the store;
             //    2 CTAs per SM.  Fastest per stream (146 K cycles per wave against 234 K), so it takes every batch
-            //    that fits its 2 x SMs CTA slots -- and all multi-CTA-per-stream work.
+            //    that fits its 2 x SMs CTA slots, and the heads and tails of run_split.
             //  * inflate_parallel_kernel (round 1): 16 KiB output image, window read back from HBM/L2, 4 CTAs per
             //    SM.  Slower per stream, but twice the streams in flight hide its barrier phases once a batch
             //    exceeds the wave kernel's slots.
             //  * inflate_cells_kernel (round 2, second half): the same waves, but the LZ77 half works on 16-bit cells in
-            //    shared memory resolved by pointer jumping; no window in shared memory, 3 CTAs per SM.  Waves that
-            //    expand beyond ~16 KB are cut, so it is meant for streams that expand less than ~2x per wave
-            //    (photographic PNG data); flat graphics stay with the ring kernel.
+            //    shared memory resolved by pointer jumping; no window in shared memory, 3 CTAs per SM.  It decodes the
+            //    segments of run_segments; whole streams go to it only in inflate mode 6.
+            // The automatic choice goes by how many streams there are to keep the SMs busy.
             const size_t wave_slots = (size_t)ctx->sm_count * WV_CTAS_PER_SM;
             const size_t streams_in_flight = std::max(par.size(), ctx->peer_streams);   // (lanes: the chunks of a host batch run side by side)
-            enum { ENG_PARALLEL = 0, ENG_WAVE = 1, ENG_CELLS = 2 };
-            int engine = streams_in_flight <= wave_slots ? ENG_WAVE : ENG_PARALLEL;
-            if (ctx->inflate_mode == 0 || ctx->inflate_mode == 5) {
-                uint64_t in_bytes = 0, out_bytes = 0;
-                for (uint32_t i : par) { in_bytes += h_jobs[i].src_len; out_bytes += h_jobs[i].dst_cap; }
-                if (ctx->cells_auto && out_bytes <= in_bytes * 9 / 4) engine = ENG_CELLS;
-            }
+            Engine engine = streams_in_flight <= wave_slots ? ENG_WAVE : ENG_PARALLEL;
             if (ctx->inflate_mode == 3) engine = ENG_WAVE;
             if (ctx->inflate_mode == 4) engine = ENG_PARALLEL;
             if (ctx->inflate_mode == 6) engine = ENG_CELLS;
-            const bool use_wave = engine == ENG_WAVE;
             ctx->last_engine = engine;
-            const uint64_t bitmap_words = engine == ENG_CELLS ? 8 : use_wave ? wv_bitmap_words(max_cap) : par_bitmap_words(max_cap);
-            const uint64_t stride = engine == ENG_CELLS ? CL_SCRATCH : use_wave ? wv_scratch_stride(bitmap_words) : par_scratch_stride(bitmap_words);
-            unsigned grid = (unsigned)std::min<size_t>(par.size(), engine == ENG_CELLS ? (size_t)ctx->sm_count * CL_CTAS_PER_SM
-                                                                   : use_wave         ? wave_slots
-                                                                                      : (size_t)ctx->sm_count * PAR_CTAS_PER_SM);
-            size_t need = (size_t)stride * grid + 256;
-            // The per-CTA "unresolved" bitmaps must be all-zero when a launch starts; the kernels
-            // leave them clean.  A different stride moves the bitmaps onto bytes that held copy
-            // lists before, and a fresh allocation is garbage: zero the whole arena in both cases.
-            if (need > ctx->d_scratch.cap || stride != ctx->scratch_stride) {
-                CU(ctx->d_scratch.reserve(need));
-                CU(cudaMemsetAsync(ctx->d_scratch.p, 0, ctx->d_scratch.cap, ctx->stream));
-                ctx->scratch_stride = stride;
-            }
-            uint32_t* ticket = (uint32_t*)((char*)ctx->d_scratch.p + (size_t)stride * grid);
-            CU(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), ctx->stream));
-            if (!hooked)
-                if (int rc = before_first_launch()) return rc;
-            hooked = true;
-            if (engine == ENG_CELLS) {
-                WvParams pp{};
-                pp.scratch = ctx->d_scratch.as<uint8_t>();
-                pp.scratch_stride = stride;
-                pp.ticket = ticket;
-                pp.jobs = d_jobs;
-                pp.results = d_results;
-                pp.order = d_order;
-                pp.count = (int)par.size();
-                inflate_cells_kernel<<<grid, WV_THREADS, sizeof(ClShared), ctx->stream>>>(pp);
-            } else if (use_wave) {
-                WvParams pp;
-                pp.bitmap_words = bitmap_words;
-                pp.scratch_stride = stride;
-                pp.ticket = ticket;
-                pp.jobs = d_jobs;
-                pp.results = d_results;
-                pp.order = d_order;
-                pp.scratch = ctx->d_scratch.as<uint8_t>();
-                pp.count = (int)par.size();
-                inflate_wave_kernel<<<grid, WV_THREADS, sizeof(WvShared), ctx->stream>>>(pp);
-            } else {
-                ParParams pp;
-                pp.bitmap_words = bitmap_words;
-                pp.scratch_stride = stride;
-                pp.ticket = ticket;
-                pp.jobs = d_jobs;
-                pp.results = d_results;
-                pp.order = d_order;
-                pp.scratch = ctx->d_scratch.as<uint8_t>();
-                pp.count = (int)par.size();
-                if (par.size() <= (size_t)ctx->sm_count * 3)
-                    inflate_parallel_kernel3<<<grid, PAR_THREADS, sizeof(ParShared), ctx->stream>>>(pp);
-                else
-                    inflate_parallel_kernel<<<grid, PAR_THREADS, sizeof(ParShared), ctx->stream>>>(pp);
-            }
-            ctx->launches++;
+            const size_t engine_slots = engine == ENG_CELLS  ? (size_t)ctx->sm_count * CL_CTAS_PER_SM
+                                        : engine == ENG_WAVE ? wave_slots
+                                                             : (size_t)ctx->sm_count * PAR_CTAS_PER_SM;
+            if (int rc = launch_waves(ctx, engine, d_jobs, d_results, d_order, par.size(), (unsigned)std::min(par.size(), engine_slots),
+                                      max_cap, nullptr, before_first_launch))
+                return rc;
         }
-        if (!hooked)
-            if (int rc = before_first_launch()) return rc;
+        if (int rc = before_first_launch()) return rc;
         if (!ser.empty()) {
             inflate_serial_kernel<<<(unsigned)ser.size(), 32, 0, ctx->stream>>>(d_jobs, d_results, d_order + par.size(),
                                                                                  (int)ser.size());
@@ -941,8 +908,6 @@ int run_over_lanes(pngb200_ctx* ctx, size_t count, int memspace, BytesOf bytes_o
         workers.emplace_back([&, l]() {
             pngb200_ctx* lane = ctx->lanes[l];
             lane->inflate_mode = ctx->inflate_mode;
-            lane->cells_auto = ctx->cells_auto;
-            lane->cells_segments = ctx->cells_segments;
             lane->parallel_threshold = ctx->parallel_threshold;
             lane->peer_streams = count;
             for (size_t c = l; c < nchunks; c += kLanes) {
@@ -1008,9 +973,7 @@ pngb200_ctx* pngb200_ctx_create(int device)
     ctx->device = device;
     ctx->sm_count = prop.multiProcessorCount;
     ctx->device_bytes = prop.totalGlobalMem;
-    if (const char* v = getenv("PNGB200_CELLS_AUTO")) ctx->cells_auto = atoi(v) != 0;   // tuning overrides, read once per context
-    if (const char* v = getenv("PNGB200_CELLS_SEGMENTS")) ctx->cells_segments = atoi(v) != 0;
-    if (const char* v = getenv("PNGB200_SPLIT")) ctx->split = atoi(v) != 0;
+    if (const char* v = getenv("PNGB200_SPLIT")) ctx->split = atoi(v) != 0;   // tuning overrides, read once per context
     if (const char* v = getenv("PNGB200_PLAN_SLOTS")) ctx->plan_slots = (size_t)std::max(0, atoi(v));
     DeviceGuard guard(device);
     if (cudaFuncSetAttribute(deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DfShared)) != cudaSuccess) {
@@ -1202,21 +1165,10 @@ int pngb200_inflate_batch(pngb200_ctx* ctx, pngb200_stream_desc* s, size_t count
                 CU(cudaMemcpyAsync(ctx->d_in.as<uint8_t>() + in_off[i], s[i].src, s[i].src_len,
                                    cudaMemcpyHostToDevice, ctx->stream));
     }
-    for (size_t i = 0; i < count; ++i) {
+    for (size_t i = 0; i < count; ++i) {   // no scratch to borrow: streams are not cut in two
         bool host = memspace == PNGB200_MEM_HOST;
-        jobs[i].src = host ? ctx->d_in.as<uint8_t>() + in_off[i] : s[i].src;
-        jobs[i].src_len = s[i].src_len;
-        jobs[i].dst = host ? ctx->d_out.as<uint8_t>() + out_off[i] : s[i].dst;
-        jobs[i].dst_cap = s[i].dst_cap;
-        jobs[i].start_bit = 0;
-        jobs[i].start_out = 0;
-        jobs[i].format = s[i].format;
-        jobs[i].phase = 0;
-        jobs[i].stop_bit = 0;
-        jobs[i].symbolic = 0;
-        jobs[i].may_switch = 0;
-        jobs[i].scratch = nullptr;   // no buffer to borrow: streams are not cut in two
-        jobs[i].scratch_cap = 0;
+        jobs[i] = whole_stream_job(host ? ctx->d_in.as<uint8_t>() + in_off[i] : s[i].src, s[i].src_len,
+                                   host ? ctx->d_out.as<uint8_t>() + out_off[i] : s[i].dst, s[i].dst_cap, s[i].format);
     }
     CU(cudaMemcpyAsync(ctx->d_jobs.p, jobs, sizeof(StreamJob) * count, cudaMemcpyHostToDevice, ctx->stream));
     int rc = run_inflate(ctx, jobs, count);
@@ -1289,21 +1241,16 @@ int pngb200_decode_batch_enqueue(pngb200_ctx* ctx, pngb200_image_desc* im, size_
     }
     StreamJob* jobs = ctx->h_jobs.as<StreamJob>();
     for (size_t i = 0; i < count; ++i) {
-        jobs[i].src = host ? ctx->d_in.as<uint8_t>() + in_off[i] : im[i].idat;
-        jobs[i].src_len = im[i].idat_len;
-        jobs[i].dst = ctx->d_filtered.as<uint8_t>() + f_off[i];
-        jobs[i].dst_cap = geo[i].filtered + 16;  // room to notice extraneous image data
-        jobs[i].start_bit = 0;
-        jobs[i].start_out = 0;
-        jobs[i].format = im[i].format;
-        jobs[i].phase = 0;
-        jobs[i].stop_bit = 0;
-        jobs[i].symbolic = 0;
-        jobs[i].may_switch = 0;
+        jobs[i] = whole_stream_job(host ? ctx->d_in.as<uint8_t>() + in_off[i] : im[i].idat, im[i].idat_len,
+                                   ctx->d_filtered.as<uint8_t>() + f_off[i],
+                                   geo[i].filtered + 16,   // room to notice extraneous image data
+                                   im[i].format);
         // the pixel buffer is dead until unfilter writes it: a stream cut in two keeps its tail's symbols there
         // (host batches run lanes side by side and are not cut)
-        jobs[i].scratch = host ? nullptr : im[i].pixels;
-        jobs[i].scratch_cap = host ? 0 : im[i].pixels_cap;
+        if (!host) {
+            jobs[i].scratch = im[i].pixels;
+            jobs[i].scratch_cap = im[i].pixels_cap;
+        }
     }
     CU(cudaMemcpyAsync(ctx->d_jobs.p, jobs, sizeof(StreamJob) * count, cudaMemcpyHostToDevice, ctx->stream));
     int rc = run_inflate(ctx, jobs, count);
@@ -1933,17 +1880,10 @@ int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
     if (rc != PNGB200_OK) return rc;
     for (;;) {
         StreamJob* job = (StreamJob*)((char*)z->h_res.p + sizeof(StreamResult));
-        job->src = z->d_in.as<uint8_t>();
-        job->src_len = z->input.size();
-        job->dst = z->d_out.as<uint8_t>();
-        job->dst_cap = z->d_out.cap;
+        *job = whole_stream_job(z->d_in.as<uint8_t>(), z->input.size(), z->d_out.as<uint8_t>(), z->d_out.cap, z->format);
         job->start_bit = z->resume_bit;
         job->start_out = z->resume_out;
-        job->format = z->format;
         job->phase = (int32_t)z->phase;
-        job->stop_bit = 0;
-        job->symbolic = 0;
-        job->may_switch = 0;
         CU(cudaMemcpyAsync(z->d_job.p, job, sizeof(StreamJob), cudaMemcpyHostToDevice, ctx->stream));
         CU(cudaMemsetAsync(z->d_res.p, 0, sizeof(StreamResult), ctx->stream));
         // A push with a lot of undecoded input goes through the intra-stream parallel kernel (one CTA: ~25 x the
@@ -1951,30 +1891,12 @@ int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
         // at the last completed block boundary.
         const uint64_t pending = z->input.size() - std::min<uint64_t>(z->input.size(), z->resume_bit >> 3);
         if (pending >= (64u << 10)) {
-            const uint64_t bitmap_words = wv_bitmap_words(job->dst_cap);
-            const uint64_t stride = wv_scratch_stride(bitmap_words);
-            const size_t   need = (size_t)stride + 256;
-            if (need > ctx->d_scratch.cap || stride != ctx->scratch_stride) {   // (same convention as run_inflate: bitmaps start zeroed)
-                CU(ctx->d_scratch.reserve(need));
-                CU(cudaMemsetAsync(ctx->d_scratch.p, 0, ctx->d_scratch.cap, ctx->stream));
-                ctx->scratch_stride = stride;
-            }
-            uint32_t* ticket = (uint32_t*)((char*)ctx->d_scratch.p + (size_t)stride);
-            CU(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), ctx->stream));
-            WvParams pp;
-            pp.bitmap_words = bitmap_words;
-            pp.scratch_stride = stride;
-            pp.ticket = ticket;
-            pp.jobs = z->d_job.as<StreamJob>();
-            pp.results = z->d_res.as<StreamResult>();
-            pp.order = nullptr;
-            pp.scratch = ctx->d_scratch.as<uint8_t>();
-            pp.count = 1;
-            inflate_wave_kernel<<<1, WV_THREADS, sizeof(WvShared), ctx->stream>>>(pp);
+            rc = launch_waves(ctx, ENG_WAVE, z->d_job.as<StreamJob>(), z->d_res.as<StreamResult>(), nullptr, 1, 1, job->dst_cap, nullptr);
+            if (rc != PNGB200_OK) return rc;
         } else {
             inflate_serial_kernel<<<1, 32, 0, ctx->stream>>>(z->d_job.as<StreamJob>(), z->d_res.as<StreamResult>(), nullptr, 1);
+            ctx->launches++;
         }
-        ctx->launches++;
         CU(cudaGetLastError());
         CU(cudaMemcpyAsync(z->h_res.p, z->d_res.p, sizeof(StreamResult), cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));

@@ -1,13 +1,11 @@
-// Host build of the segmented-stream pipeline (block_search_kernel, inflate_wave_kernel in symbolic mode,
+// Host build of the segmented-stream pipeline (block_search_kernel, inflate_cells_kernel in symbolic mode,
 // window_propagate_kernel, marker_resolve_kernel) under the SIMT emulator: test infrastructure.  The driver
 // below restates run_segments() of pngb200_api.cu without the CUDA runtime.
 #define PNGB200_EMU 1
 #include "../../swift-png_b200/csrc/inflate_wave.cuh"
 #include "../../swift-png_b200/csrc/block_search.cuh"
 #include "../../swift-png_b200/csrc/inflate_segments.cuh"
-#ifdef EMU_SEG_CELLS
 #include "../../swift-png_b200/csrc/inflate_cells.cuh"
-#endif
 
 using namespace pngb200;
 
@@ -27,7 +25,6 @@ extern "C" int emu_inflate_segmented(const uint8_t* src, uint64_t len, uint8_t* 
     const size_t n = at.size();
     std::vector<StreamJob> sg(n);
     std::vector<std::vector<uint16_t>> sym(n);
-    uint64_t max_cap = 0;
     for (size_t k = 0; k < n; ++k) {
         const uint64_t end = k + 1 < n ? at[k + 1] : bits;
         StreamJob s{};
@@ -38,7 +35,6 @@ extern "C" int emu_inflate_segmented(const uint8_t* src, uint64_t len, uint8_t* 
         s.dst_cap = (uint64_t)((double)cap * 1.5 * (double)(end - at[k]) / (double)bits) + (64u << 10);
         sym[k].assign(s.dst_cap + 64, 0xDEAD);
         s.dst = (uint8_t*)sym[k].data();
-        max_cap = std::max(max_cap, s.dst_cap);
         sg[k] = s;
     }
     std::vector<StreamResult> sr(n);
@@ -47,18 +43,10 @@ extern "C" int emu_inflate_segmented(const uint8_t* src, uint64_t len, uint8_t* 
     WvParams P{};
     P.jobs = sg.data(); P.results = sr.data(); P.order = nullptr; P.ticket = &ticket; P.count = (int)n;
     const unsigned grid = (unsigned)std::min<size_t>(n, 3);   // fewer CTAs than segments: the ticket loop is exercised
-#ifdef EMU_SEG_CELLS
     P.scratch_stride = CL_SCRATCH;
     std::vector<uint8_t> scratch(P.scratch_stride * grid + 256, 0);
     P.scratch = scratch.data();
     simt::launch(grid, WV_THREADS, sizeof(ClShared), [&]() { inflate_cells_kernel(P); });
-#else
-    P.bitmap_words = wv_bitmap_words(max_cap);
-    P.scratch_stride = wv_scratch_stride(P.bitmap_words);
-    std::vector<uint8_t> scratch(P.scratch_stride * grid + 256, 0);
-    P.scratch = scratch.data();
-    simt::launch(grid, WV_THREADS, sizeof(WvShared), [&]() { inflate_wave_kernel(P); });
-#endif
     *segments_used = (uint32_t)n;
     bool ok = true;
     uint64_t total = 0;

@@ -142,18 +142,11 @@ def test_tiny_and_empty(lib):
 
 
 # ---- more than one CTA per stream: block search + symbolic segments + window propagation + marker resolve ----
-@pytest.fixture(scope="module", params=["wave", "cells"])
-def seglib(request):
-    """the segment pipeline with inflate_wave_kernel (shipped) and with inflate_cells_kernel decoding the segments"""
-    if request.param == "cells":
-        import subprocess
-        here = os.path.join(os.path.dirname(__file__), "emu")
-        lib = os.path.join(here, "libemu_inflate_segments_cells.so")
-        subprocess.run(["g++", "-O1", "-g", "-std=c++17", "-shared", "-fPIC", "-I" + here, "-Wno-attributes", "-DEMU_SEG_CELLS",
-                        "-o", lib, os.path.join(here, "emu_inflate_segments.cpp")], check=True)
-        L = C.CDLL(lib)
-    else:
-        L = emu.load("emu_inflate_segments")
+@pytest.fixture(scope="module", params=["cells"])
+def seglib():
+    """the segment pipeline, with inflate_cells_kernel decoding the segments (as run_segments does; the test ids name
+    the engine)"""
+    L = emu.load("emu_inflate_segments")
     L.emu_inflate_segmented.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_int, C.c_uint32, C.c_uint64,
                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
     return L
