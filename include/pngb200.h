@@ -232,15 +232,38 @@ int pngb200_filter_batch(pngb200_ctx* ctx, pngb200_filter_desc* images, size_t c
  * PNG.VA.swift, PNG.Color.swift, over the convolve / deconvolve closures of Sources/PNG/PNG.swift:149-1285.
  * The unpack is inside the reference's own timed decode loop (Benchmarks/Decompression/Swift/Main.swift:105-106).
  * For rgba8 -> RGBA<UInt8> and va8 -> VA<UInt8> the unpacked array IS PNG.Image.storage, byte for
- * byte, so pngb200_decode_batch's output needs no second pass. */
+ * byte, so pngb200_decode_batch's output needs no second pass.
+ *
+ * RGBA32 / RGBA64 / VA32 / VA64 are the UInt32 / UInt64 specialisations of the same types
+ * (PNG.RGBA.swift:253-257; Swift's UInt is UInt64 on every 64-bit platform): 16 / 32 / 8 / 16 bytes
+ * per pixel, chroma key -> alpha 0, bgr samples swapped, VA keeps r, exactly as at 8 and 16 bits.
+ * V8 ... V64 are the scalar targets image.unpack(as: T.self) / PNG.Image(packing: [T], ...) with
+ * T = UInt8 ... UInt64 (PNG.Image.swift:681-833, 1079-1145), 1 / 2 / 4 / 8 bytes per pixel:
+ *   unpack: v of v and va, r of rgb and rgba (c.2 of bgr8 / bgra8), palette[i].r widened from 8 bits;
+ *           chroma keys are ignored (the scalar target has no alpha);
+ *   pack:   v -> (v), va -> (v, T.max), rgb / bgr -> (v, v, v), rgba / bgra -> (v, v, v, T.max), each
+ *           narrowed to the format's depth; indexed formats store the first palette entry equal to
+ *           (v8, v8, v8, 255) with v8 = v >> (T.bitWidth - 8), else 0 (the default indexer, :1126-1145).
+ * With PNGB200_MEM_DEVICE, `pixels` must be aligned to min(bytes per pixel, 16): RGBA64 needs 16 bytes,
+ * V8 needs none. */
 typedef enum pngb200_target {
-    PNGB200_TARGET_RGBA8 = 0, PNGB200_TARGET_RGBA16 = 1, PNGB200_TARGET_VA8 = 2, PNGB200_TARGET_VA16 = 3
+    PNGB200_TARGET_RGBA8 = 0, PNGB200_TARGET_RGBA16 = 1, PNGB200_TARGET_VA8 = 2, PNGB200_TARGET_VA16 = 3,
+    PNGB200_TARGET_RGBA32 = 4, PNGB200_TARGET_RGBA64 = 5, PNGB200_TARGET_VA32 = 6, PNGB200_TARGET_VA64 = 7,
+    PNGB200_TARGET_V8 = 8, PNGB200_TARGET_V16 = 9, PNGB200_TARGET_V32 = 10, PNGB200_TARGET_V64 = 11
 } pngb200_target;
 /* applied per pixel after unpacking: .premultiplied / .straightened (PNG.RGBA.swift:115-121, 163-169),
- * or premultiplied(as: UInt8.self) / straightened(as: UInt8.self) of a 16-bit target (:141-155, 187-201) */
+ * or premultiplied(as: U.self) / straightened(as: U.self) with U = UInt8 / UInt16 / UInt32
+ * (PNG.RGBA.swift:146-206, PNG.VA.swift:79, 120): shift = T.bitWidth - U.bitWidth,
+ * q = T.max / (T.max >> shift), every component including alpha requantised through U.
+ * Valid combinations: a scalar target (V8 ... V64) takes only ASIS; _AS{U} needs an RGBA or VA target
+ * whose T is wider than U (AS8: 16, 32, 64 bits; AS16: 32, 64; AS32: 64).  Anything else is
+ * PNGB200_ERR_BAD_ARGUMENT before any work.  At 64 bits the products are full 128-bit, and
+ * straightening saturates at T.max where the reference's dividingFullWidth traps. */
 typedef enum pngb200_alpha_mode {
     PNGB200_ALPHA_ASIS = 0, PNGB200_ALPHA_PREMULTIPLIED = 1, PNGB200_ALPHA_STRAIGHTENED = 2,
-    PNGB200_ALPHA_PREMULTIPLIED_AS8 = 3, PNGB200_ALPHA_STRAIGHTENED_AS8 = 4
+    PNGB200_ALPHA_PREMULTIPLIED_AS8 = 3, PNGB200_ALPHA_STRAIGHTENED_AS8 = 4,
+    PNGB200_ALPHA_PREMULTIPLIED_AS16 = 5, PNGB200_ALPHA_STRAIGHTENED_AS16 = 6,
+    PNGB200_ALPHA_PREMULTIPLIED_AS32 = 7, PNGB200_ALPHA_STRAIGHTENED_AS32 = 8
 } pngb200_alpha_mode;
 /* PNG.Format (Sources/PNG/Formats/PNG.Format.swift:6-43) as these kernels see it */
 typedef struct pngb200_pixel_format {
@@ -255,7 +278,7 @@ typedef struct pngb200_pixel_format {
 typedef struct pngb200_color_desc {
     void*                storage;      /* PNG.Image.storage: unpack reads it, pack writes it */
     size_t               storage_len;  /* bytes (capacity for pack) */
-    void*                pixels;       /* [RGBA<T>] / [VA<T>]: native-endian T components, aligned to the pixel size */
+    void*                pixels;       /* [RGBA<T>] / [VA<T>] / [T]: native-endian T components, aligned to min(pixel size, 16) */
     size_t               pixels_len;   /* bytes (capacity for unpack) */
     uint64_t             count;        /* number of pixels */
     pngb200_pixel_format format;

@@ -120,9 +120,14 @@ class EncodeDesc(C.Structure):
 
 
 TARGET_RGBA8, TARGET_RGBA16, TARGET_VA8, TARGET_VA16 = 0, 1, 2, 3
+TARGET_RGBA32, TARGET_RGBA64, TARGET_VA32, TARGET_VA64 = 4, 5, 6, 7
+TARGET_V8, TARGET_V16, TARGET_V32, TARGET_V64 = 8, 9, 10, 11  # image.unpack(as: UInt8.self) ... UInt64
 ALPHA_ASIS, ALPHA_PREMULTIPLIED, ALPHA_STRAIGHTENED, ALPHA_PREMULTIPLIED_AS8, ALPHA_STRAIGHTENED_AS8 = range(5)
+ALPHA_PREMULTIPLIED_AS16, ALPHA_STRAIGHTENED_AS16, ALPHA_PREMULTIPLIED_AS32, ALPHA_STRAIGHTENED_AS32 = 5, 6, 7, 8
 ERR_PNG_PALETTE_INDEX = -51
-_TARGET_BYTES = {TARGET_RGBA8: 4, TARGET_RGBA16: 8, TARGET_VA8: 2, TARGET_VA16: 4}
+_TARGET_BYTES = {TARGET_RGBA8: 4, TARGET_RGBA16: 8, TARGET_VA8: 2, TARGET_VA16: 4,
+                 TARGET_RGBA32: 16, TARGET_RGBA64: 32, TARGET_VA32: 8, TARGET_VA64: 16,
+                 TARGET_V8: 1, TARGET_V16: 2, TARGET_V32: 4, TARGET_V64: 8}
 _CHANNELS = {0: 1, 2: 3, 3: 1, 4: 2, 6: 4}
 
 

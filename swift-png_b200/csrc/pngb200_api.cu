@@ -1538,16 +1538,23 @@ int run_color(pngb200_ctx* ctx, pngb200_color_desc* im, size_t count, int target
 {
     if (!ctx || (!im && count)) return PNGB200_ERR_BAD_ARGUMENT;
     if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a decode batch is pending");
-    if (target < PNGB200_TARGET_RGBA8 || target > PNGB200_TARGET_VA16 || alpha_mode < PNGB200_ALPHA_ASIS ||
-        alpha_mode > PNGB200_ALPHA_STRAIGHTENED_AS8)
+    if (target < PNGB200_TARGET_RGBA8 || target > PNGB200_TARGET_V64 || alpha_mode < PNGB200_ALPHA_ASIS ||
+        alpha_mode > PNGB200_ALPHA_STRAIGHTENED_AS32)
         return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "bad colour target / alpha mode");
-    const bool wide_target = target == PNGB200_TARGET_RGBA16 || target == PNGB200_TARGET_VA16;
-    if (alpha_mode >= PNGB200_ALPHA_PREMULTIPLIED_AS8 && !wide_target)
-        return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "premultiplied(as: UInt8) needs a 16-bit target");
+    // per target: component bits and bytes per pixel
+    static const int    kTargetBits[]  = {8, 16, 8, 16, 32, 64, 32, 64, 8, 16, 32, 64};
+    static const size_t kTargetBytes[] = {4, 8, 2, 4, 16, 32, 8, 16, 1, 2, 4, 8};
+    if (target >= PNGB200_TARGET_V8 && alpha_mode != PNGB200_ALPHA_ASIS)
+        return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a scalar target has no alpha to premultiply or straighten");
+    if (alpha_mode >= PNGB200_ALPHA_PREMULTIPLIED_AS8) {
+        const int u = alpha_mode <= PNGB200_ALPHA_STRAIGHTENED_AS8 ? 8 : alpha_mode <= PNGB200_ALPHA_STRAIGHTENED_AS16 ? 16 : 32;
+        if (kTargetBits[target] <= u)
+            return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "premultiplied(as: UInt%d) needs a target wider than %d bits", u, u);
+    }
     if (count == 0) return PNGB200_OK;
     DeviceGuard guard(ctx->device);
     const bool   host = memspace == PNGB200_MEM_HOST;
-    const size_t tpx  = target == PNGB200_TARGET_RGBA8 ? 4 : target == PNGB200_TARGET_RGBA16 ? 8 : target == PNGB200_TARGET_VA8 ? 2 : 4;
+    const size_t tpx  = kTargetBytes[target];
     std::vector<ColorJob> jobs(count);
     std::vector<size_t>   s_off(count), p_off(count), s_len(count);
     std::vector<uint32_t> palettes;
@@ -1566,7 +1573,7 @@ int run_color(pngb200_ctx* ctx, pngb200_color_desc* im, size_t count, int target
         s_len[i] = (size_t)im[i].count * ch * (f.depth == 16 ? 2 : 1);
         if (im[i].storage_len < s_len[i] || im[i].pixels_len < im[i].count * tpx)
             return set_error(ctx, PNGB200_ERR_OUTPUT_CAPACITY, "image %zu: buffer too small", i);
-        if (!host && (((uintptr_t)im[i].pixels) & (tpx - 1)))
+        if (!host && (((uintptr_t)im[i].pixels) & (std::min<size_t>(tpx, 16) - 1)))
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: pixel array is not aligned to its element size", i);
         s_off[i] = s_total, p_off[i] = p_total;
         s_total += align_up(s_len[i] + 16, 256);
@@ -1613,8 +1620,21 @@ int run_color(pngb200_ctx* ctx, pngb200_color_desc* im, size_t count, int target
     const unsigned gy = (unsigned)std::min<size_t>(count, 65535);
     const uint64_t tiles = std::max<uint64_t>(1, (most + COLOR_TILE - 1) / COLOR_TILE);
     const unsigned gx = (unsigned)std::min<uint64_t>(tiles, std::max<uint64_t>(1, (uint64_t)ctx->sm_count * 8 / gy));
-    if (unpack) unpack_kernel<<<dim3(gx, gy), COLOR_THREADS, 0, ctx->stream>>>(p);
-    else pack_kernel<<<dim3(gx, gy), COLOR_THREADS, 0, ctx->stream>>>(p);
+    // the four 8/16-bit targets share one kernel per direction; each wider or scalar target has its own
+    using ColorKernel = void (*)(ColorParams);
+    static const ColorKernel kUnpack[] = {
+        unpack_kernel, unpack_kernel, unpack_kernel, unpack_kernel,
+        unpack_wide_kernel<32, COLOR_RGBA>, unpack_wide_kernel<64, COLOR_RGBA>,
+        unpack_wide_kernel<32, COLOR_VA>, unpack_wide_kernel<64, COLOR_VA>,
+        unpack_wide_kernel<8, COLOR_V>, unpack_wide_kernel<16, COLOR_V>,
+        unpack_wide_kernel<32, COLOR_V>, unpack_wide_kernel<64, COLOR_V>};
+    static const ColorKernel kPack[] = {
+        pack_kernel, pack_kernel, pack_kernel, pack_kernel,
+        pack_wide_kernel<32, COLOR_RGBA>, pack_wide_kernel<64, COLOR_RGBA>,
+        pack_wide_kernel<32, COLOR_VA>, pack_wide_kernel<64, COLOR_VA>,
+        pack_wide_kernel<8, COLOR_V>, pack_wide_kernel<16, COLOR_V>,
+        pack_wide_kernel<32, COLOR_V>, pack_wide_kernel<64, COLOR_V>};
+    (unpack ? kUnpack : kPack)[target]<<<dim3(gx, gy), COLOR_THREADS, 0, ctx->stream>>>(p);
     ctx->launches++;
     CU(cudaGetLastError());
     if (host)
