@@ -49,14 +49,8 @@
 
 namespace pngb200 {
 
-#ifndef CL_CTAS
-#define CL_CTAS 3
-#endif
-#ifndef CL_NSLOTS
-#define CL_NSLOTS 16000
-#endif
-constexpr int      CL_CTAS_PER_SM = CL_CTAS;
-constexpr uint32_t CL_SLOTS       = CL_NSLOTS;             // cell slots (16-bit), <= 16384 (14-bit cell index)
+constexpr int      CL_CTAS_PER_SM = 3;
+constexpr uint32_t CL_SLOTS       = 16000;                 // cell slots (16-bit), <= 16384 (14-bit cell index)
 constexpr uint32_t CL_CAP         = CL_SLOTS - 16;         // largest wave output (the first slots mirror dst's 16-byte phase)
 constexpr uint32_t CL_INWAVE      = 0xc000u;               // cell >= this: pointer to cell (cell & 0x3fff)
 constexpr uint32_t CL_WINDOW_BIAS = 0x8100u;               // 0x100 <= cell < 0x8100: window position cell - 0x8100

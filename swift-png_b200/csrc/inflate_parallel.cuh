@@ -41,23 +41,15 @@
 namespace pngb200 {
 namespace par {
 
-// CTA shape (tunable at compile time: more, smaller CTAs hide each other's barrier phases)
-#ifndef PAR_T
-#define PAR_T 256
-#define PAR_C 4
-#define PAR_O 16384
-#endif
-constexpr int      PAR_THREADS      = PAR_T;
-constexpr int      PAR_CTAS_PER_SM  = PAR_C;
+// CTA shape (more, smaller CTAs hide each other's barrier phases)
+constexpr int      PAR_THREADS      = 256;
+constexpr int      PAR_CTAS_PER_SM  = 4;
 constexpr int      PAR_WARPS        = PAR_THREADS / 32;
-#ifndef PAR_S
-#define PAR_S 256
-#endif
-constexpr uint32_t PAR_SUB_BITS     = PAR_S;
+constexpr uint32_t PAR_SUB_BITS     = 256;
 constexpr uint32_t PAR_SUB_WORDS    = PAR_SUB_BITS / 32;
 constexpr uint32_t PAR_WAVE_WORDS   = PAR_THREADS * PAR_SUB_WORDS + 8;
 constexpr uint32_t PAR_SMEM_WORDS   = PAR_WAVE_WORDS + PAR_WAVE_WORDS / 8 + 1;
-constexpr uint32_t PAR_OUT_BYTES    = PAR_O;                         // wave output image in smem
+constexpr uint32_t PAR_OUT_BYTES    = 16384;                         // wave output image in smem
 constexpr uint32_t PAR_BITMAP_WORDS = PAR_OUT_BYTES / 32;
 constexpr uint32_t PAR_LIST_CAP     = PAR_THREADS * (PAR_SUB_BITS / 2);  // >= copies per wave (2 bits min each)
 constexpr uint64_t PAR_MAX_WAVE_OUT = (uint64_t)PAR_LIST_CAP * 258;

@@ -58,11 +58,8 @@
 
 namespace pngb200 {
 
-#ifndef WV_CTAS
-#define WV_CTAS 2
-#endif
 constexpr int      WV_THREADS      = 256;
-constexpr int      WV_CTAS_PER_SM  = WV_CTAS;
+constexpr int      WV_CTAS_PER_SM  = 2;
 constexpr int      WV_WARPS        = WV_THREADS / 32;
 constexpr uint32_t WV_SUB_BITS     = 256;
 constexpr uint32_t WV_BITS         = WV_THREADS * WV_SUB_BITS;          // 65536 bits per wave
@@ -76,9 +73,7 @@ constexpr uint32_t WV_LIST_CAP     = WV_BITS / 2 + 64;                  // >= co
 constexpr uint64_t WV_MAX_WAVE_OUT = (uint64_t)WV_LIST_CAP * 258;
 constexpr uint32_t WV_HDR_WORDS    = 192;                               // block header staging (<= 566 bytes)
 constexpr uint32_t ADLER_MOD32     = 65521;
-#ifndef WV_POLL_NS
-#define WV_POLL_NS 20
-#endif
+constexpr unsigned WV_POLL_NS      = 20;
 constexpr uint32_t WV_WALK_K       = 8;                                 // tokens per walk in round 0 (doubles)
 
 // cost model instrumentation (emulator builds only): loop trips per thread and per warp (max over lanes)

@@ -795,7 +795,6 @@ int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
             auto nb = [&](uint32_t i) { return (fast[i].height + 31) / 32; };
             std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return nb(a) > nb(b); });
             const uint32_t maxb = nb(idx[0]);
-#ifndef PNGB200_WAVE_IMAGE_MAJOR   // (tuning builds: the round-2a order)
             if (maxb <= 4096) {
                 std::vector<ImageJob> sorted(fast.size());
                 for (size_t i = 0; i < idx.size(); ++i) sorted[i] = fast[idx[i]];
@@ -812,9 +811,6 @@ int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
                     level_start[b + 1] = level_start[b] + (uint32_t)alive;
                 }
             }
-#else
-            (void)maxb;
-#endif
         }
         size_t jb = sizeof(ImageJob) * fast.size(), bb = sizeof(uint32_t) * band_base.size();
         size_t lb = sizeof(uint32_t) * level_start.size();

@@ -12,8 +12,8 @@
 //   "previous row").  Bands are pipelined the same way through HBM/L2: the last row of band k is
 //   the previous row of band k+1, published chunk-by-chunk with a progress counter.  Bands are
 //   handed out by an atomic ticket in row order, so a band's predecessor is always already
-//   running (no deadlock whatever the residency).  Each lane reads its own row with 16-byte
-//   loads (L1 keeps the 128-byte line for the next 7 chunks) and writes 16-byte stores.
+//   running (no deadlock whatever the residency).  Each lane stages its own row through a
+//   shared-memory ring in 16-byte chunks (see WAVE_DEPTH) and writes 16-byte stores.
 //
 // unfilter_generic_kernel: every other format (Adam7, 1/2/4-bit samples); one CTA per image.
 #pragma once
@@ -127,64 +127,17 @@ struct WaveParams {
                                 // -DDUMP_FILTERED_SCANLINES view of a decode, PNG.Decoder.swift:96-98,128); may be null
 };
 
-#ifndef PNGB200_WAVE_WARPS
-#define PNGB200_WAVE_WARPS 4
-#endif
-constexpr int WAVE_WARPS   = PNGB200_WAVE_WARPS;
-#ifndef PNGB200_WAVE_PUBLISH
-#define PNGB200_WAVE_PUBLISH 8
-#endif
-constexpr int WAVE_PUBLISH = PNGB200_WAVE_PUBLISH;  // publish progress every this many chunks
-#ifndef PNGB200_WAVE_POLL_NS
-#define PNGB200_WAVE_POLL_NS 64
-#endif
-// A band that has caught up with the band above waits until that band is WAVE_LAG chunks ahead again, not just one:
-// right behind its producer a band pays two L2 round trips per chunk (the progress word, then the row-above chunk,
-// which cannot be prefetched before it is published).
-#ifndef PNGB200_WAVE_LAG
-#define PNGB200_WAVE_LAG 1
-#endif
-constexpr uint32_t WAVE_LAG = PNGB200_WAVE_LAG;
-// Lane 0's "previous row" is the last row of the band above, written by another warp.  Fetched one step ahead in
-// registers (round 2a) its L2 round trip sat on the warp's critical path at every step (on the
-// first use of that value).  WAVE_ABOVE: lane 0 stages the aligned chunks of that row through a 32-slot ring with
-// the same cp.async groups as its own row, two blocks of 8 ahead, as far as the band above has published them.
-#ifndef PNGB200_WAVE_ABOVE
-#define PNGB200_WAVE_ABOVE 0
-#endif
-constexpr int WAVE_ABOVE = PNGB200_WAVE_ABOVE;
-// Every lane asks L2 for the 128-byte line of its row that lies WAVE_L2PF bytes ahead of the chunk it is staging (one
-// prefetch.global.L2 per 8 chunks): lookahead beyond the shared-memory ring without paying for it in resident warps.
-#ifndef PNGB200_WAVE_L2PF
-#define PNGB200_WAVE_L2PF 0
-#endif
-constexpr int WAVE_L2PF = PNGB200_WAVE_L2PF;
-__device__ __forceinline__ void prefetch_l2(const void* p)
-{
-#ifndef PNGB200_EMU
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-#endif
-}
-
 // Asynchronous staging of a lane's own row (cp.async = LDGSTS: global -> shared memory without a register in
-// between).  Every lane keeps a private ring of WAVE_DEPTH aligned 16-byte chunks of its row in shared memory and
-// refills it in BURSTS of WAVE_BURST chunks (= one 128-byte line of its row at a time, two bursts ahead of the
-// arithmetic).  A warp touches 32 rows that lie pitch + 1 bytes apart; fetched 16 bytes per row and step (round 2,
-// first half: WAVE_BURST 1) every DRAM access was a lone 32-byte sector in its own DRAM page -- ~1.7 TB/s whatever the
-// prefetch depth.  A burst asks for the four sectors of a line back to back, so the memory controller serves them
-// from one row activation.  The reconstructed chunks leave the same way: WAVE_BURST chunks per lane collect in a
-// second small ring and are stored as one run of consecutive 16-byte stores (a full line per row for L2 to merge).
-#ifndef PNGB200_WAVE_BURST
-#define PNGB200_WAVE_BURST 1
-#endif
-constexpr int WAVE_BURST = PNGB200_WAVE_BURST;                 // chunks per refill (1: one chunk per step, as in round 2a)
-#ifndef PNGB200_WAVE_DEPTH1
-#define PNGB200_WAVE_DEPTH1 16
-#endif
-constexpr int WAVE_DEPTH = WAVE_BURST == 1 ? PNGB200_WAVE_DEPTH1 : 3 * WAVE_BURST;   // ring slots per lane
-constexpr int WAVE_OUT   = WAVE_BURST == 1 ? 0 : WAVE_BURST;   // output chunks collected per lane before they are stored
-constexpr int WAVE_OUTM  = WAVE_OUT ? WAVE_OUT : 1;           // (modulus that is never zero)
-constexpr size_t WAVE_SMEM = sizeof(uint4) * 32 * (size_t)WAVE_WARPS * (WAVE_DEPTH + (WAVE_OUT ? WAVE_OUT : 0) + (WAVE_ABOVE ? 1 : 0));
+// between).  Every lane keeps a private ring of WAVE_DEPTH aligned 16-byte chunks of its row in shared memory: the
+// first WAVE_DEPTH chunks are issued before the sweep, and step j issues chunk j + WAVE_DEPTH into the slot chunk j
+// has just left.  Reconstructed chunks are stored straight from registers.  The rings are the CTA's whole shared
+// memory (WAVE_SMEM, 32 KiB); a deeper ring, or a second one for the output or for lane 0's row above, costs resident
+// warps, and the kernel's throughput follows resident warps, not lookahead per warp (DESIGN §4.3).
+constexpr int      WAVE_WARPS   = 4;    // warps per CTA
+constexpr int      WAVE_DEPTH   = 16;   // ring slots per lane
+constexpr int      WAVE_PUBLISH = 8;    // publish progress every this many chunks
+constexpr unsigned WAVE_POLL_NS = 64;   // lane 0's back-off while the band above has not published the chunk it needs
+constexpr size_t   WAVE_SMEM    = sizeof(uint4) * 32 * (size_t)WAVE_WARPS * WAVE_DEPTH;
 __device__ __forceinline__ void cp_async16(uint4* smem, const uint4* gmem)
 {
 #ifdef PNGB200_EMU
@@ -209,7 +162,7 @@ __device__ __forceinline__ void cp_async_wait()   // at most N of this thread's 
 
 template <int BPP>
 __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_prev, uint32_t* prog_mine, uint4 (*ring)[32],
-                          uint4 (*oring)[32], uint4* aring, unsigned long long* hist)
+                          unsigned long long* hist)
 {
     const unsigned lane   = lane_id();
     const uint32_t y      = band * 32 + lane;
@@ -250,28 +203,13 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
     uint32_t seen = 0;
     uint4    upn = make_uint4(0, 0, 0, 0);  // lane 0: the chunk of the row above for the next step
     bool     upn_ok = false;
-    // lane 0, WAVE_ABOVE: aligned 16-byte chunks of the row above; chunk c lives in aring[c & 31]
-    const uint32_t ma    = above != nullptr ? (uint32_t)((uintptr_t)above & 15) : 0u;
-    const uint4*   aq    = (const uint4*)(above - ma);
-    const uint32_t nqa   = (ma + pitch + 15) >> 4;
-    uint32_t       a_cur = 0, a_prev = 0;   // aligned chunks issued so far / as of the block boundary before this one
     // input chunk k of my row is cp.async group k of this thread: WAVE_DEPTH groups are opened here, one more per
     // step, so when chunk j is consumed the groups up to j + 1 must have landed = at most WAVE_DEPTH - 2 in flight
     if (active) {
-        if (WAVE_BURST == 1) {
 #pragma unroll
-            for (int k = 0; k < WAVE_DEPTH; ++k) {
-                if (k < nq) cp_async16(&ring[k][lane], inq + k);
-                cp_async_commit();
-            }
-        } else {
-            // two bursts (chunks 0 .. 2 WAVE_BURST - 1) are on their way before the first chunk is used; burst b is
-            // cp.async group b of this thread
-#pragma unroll
-            for (int k = 0; k < 2 * WAVE_BURST; ++k) {
-                if (k < nq) cp_async16(&ring[k][lane], inq + k);
-                if ((k + 1) % WAVE_BURST == 0) cp_async_commit();
-            }
+        for (int k = 0; k < WAVE_DEPTH; ++k) {
+            if (k < nq) cp_async16(&ring[k][lane], inq + k);
+            cp_async_commit();
         }
     }
 
@@ -286,33 +224,14 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
             // the band above publishes its last row chunk by chunk; its chunk j + 1 is fetched while chunk j
             // is being used, so the L2 round trip of that load is off the warp's critical path
             up = make_uint4(0, 0, 0, 0);
-            bool staged_above = false;
-            if (WAVE_ABOVE && WAVE_BURST == 1 && active && above != nullptr && j >= 0 && j < nchunk) {
-                if (j % 8 == 0) {
-                    // once per block of 8: how far has the band above got; issue what it has published of the next
-                    // two blocks (these copies join this step's cp.async group: they have landed 8 steps from now)
-                    a_prev = a_cur;
-                    if (seen < (uint32_t)nchunk) seen = ld_volatile_u32(prog_prev);
-                    const uint32_t avail = seen >= (uint32_t)nchunk ? nqa : seen;   // aligned chunk c is complete once c + 1 <= seen
-                    const uint32_t hi = min(min(avail, (uint32_t)j + 18u), nqa);
-                    for (uint32_t c = a_cur; c < hi; ++c) cp_async16(&aring[c & 31], aq + c);
-                    a_cur = max(a_cur, hi);
-                }
-                if ((uint32_t)j + (ma ? 2u : 1u) <= a_prev) {
-                    const uint4 q0 = aring[j & 31];
-                    up = ma == 0 ? q0 : shift_bytes(q0, aring[(j + 1) & 31], ma);
-                    staged_above = true;
-                    upn_ok = false;
-                }
-            }
-            if (!staged_above && active && above != nullptr && j < nchunk) {
+            if (active && above != nullptr && j < nchunk) {
                 if (upn_ok) {
                     up = upn;
                 } else {
-                    const uint32_t want = min((uint32_t)j + WAVE_LAG, (uint32_t)nchunk);   // chunks the band above must have published
+                    const uint32_t want = min((uint32_t)j + 1u, (uint32_t)nchunk);   // chunks the band above must have published
                     while (seen < want) {
                         seen = ld_volatile_u32(prog_prev);
-                        if (seen < want) __nanosleep(PNGB200_WAVE_POLL_NS);
+                        if (seen < want) __nanosleep(WAVE_POLL_NS);
                     }
                     up = load16_any(above + 16 * (uint64_t)j, true);
                 }
@@ -327,27 +246,13 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
             }
         }
         if (active && j >= 0 && j < nchunk) {
-            if (WAVE_BURST == 1) cp_async_wait<WAVE_DEPTH - 2>();
-            else if (j % WAVE_BURST == 0) {
-                // burst j / WAVE_BURST + 2 (chunks j + 2 WAVE_BURST ...) goes into the slots the burst before this one
-                // has left; then everything but that newest group must have landed: chunks up to j + 2 WAVE_BURST - 1
-#pragma unroll
-                for (int k = 0; k < WAVE_BURST; ++k) {
-                    const int c = j + 2 * WAVE_BURST + k;
-                    if (c < nq) cp_async16(&ring[c % WAVE_DEPTH][lane], inq + c);
-                }
-                cp_async_commit();
-                cp_async_wait<1>();
-            }
+            cp_async_wait<WAVE_DEPTH - 2>();
             qcur = ring[j % WAVE_DEPTH][lane];
             const uint4 qnext = ring[(j + 1) % WAVE_DEPTH][lane];
             uint4 x = m == 0 ? qcur : shift_bytes(qcur, qnext, m);
-            if (WAVE_BURST == 1) {
-                // chunk j + WAVE_DEPTH takes the slot chunk j just left (x depends on the loads above: they are done)
-                if (j + WAVE_DEPTH < nq) cp_async16(&ring[j % WAVE_DEPTH][lane], inq + j + WAVE_DEPTH);
-                cp_async_commit();
-                if (WAVE_L2PF && (j & 7) == 0 && j + WAVE_DEPTH + WAVE_L2PF / 16 < nq) prefetch_l2(inq + j + WAVE_DEPTH + WAVE_L2PF / 16);
-            }
+            // chunk j + WAVE_DEPTH takes the slot chunk j just left (x depends on the loads above: they are done)
+            if (j + WAVE_DEPTH < nq) cp_async16(&ring[j % WAVE_DEPTH][lane], inq + j + WAVE_DEPTH);
+            cp_async_commit();
             uint4 o;
             if (BPP == 4) {
                 o.x = __vadd4(x.x, predict4(type, a1, up.x, c1, any_paeth));
@@ -384,18 +289,7 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
                 }
                 o = make_uint4(os[0], os[1], os[2], os[3]);
             }
-            if (WAVE_OUT == 0) {
-                int nbytes = (int)pitch - 16 * j;
-                store16_partial(out + 16 * (uint64_t)j, o, nbytes);
-            } else {
-                oring[j % WAVE_OUTM][lane] = o;
-                if ((j + 1) % WAVE_OUTM == 0 || j + 1 == nchunk) {
-                    const int j0 = j - j % WAVE_OUTM;
-#pragma unroll
-                    for (int k = 0; k < WAVE_OUT; ++k)
-                        if (j0 + k <= j) store16_partial(out + 16 * (uint64_t)(j0 + k), oring[k][lane], (int)pitch - 16 * (j0 + k));
-                }
-            }
+            store16_partial(out + 16 * (uint64_t)j, o, (int)pitch - 16 * j);
             mine = o;
             if (publish && (((j + 1) % WAVE_PUBLISH) == 0 || j + 1 == nchunk)) {
                 __threadfence();
@@ -409,10 +303,8 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
 
 __global__ void __launch_bounds__(WAVE_WARPS * 32) unfilter_wave_kernel(WaveParams p)
 {
-    PNGB200_DYN_SMEM(wave_smem);   // [warp][slot][lane] input rings, then [warp][slot][lane] output rings: conflict-free 16-byte accesses
-    uint4 (*ring)[32]  = reinterpret_cast<uint4 (*)[32]>(wave_smem) + (threadIdx.x >> 5) * WAVE_DEPTH;
-    uint4 (*oring)[32] = reinterpret_cast<uint4 (*)[32]>(wave_smem) + WAVE_WARPS * WAVE_DEPTH + (threadIdx.x >> 5) * WAVE_OUT;
-    uint4* aring = reinterpret_cast<uint4*>(reinterpret_cast<uint4 (*)[32]>(wave_smem) + WAVE_WARPS * (WAVE_DEPTH + WAVE_OUT) + (threadIdx.x >> 5));
+    PNGB200_DYN_SMEM(wave_smem);   // [warp][slot][lane] input rings: conflict-free 16-byte accesses
+    uint4 (*ring)[32] = reinterpret_cast<uint4 (*)[32]>(wave_smem) + (threadIdx.x >> 5) * WAVE_DEPTH;
     const unsigned lane = lane_id();
     for (;;) {
         uint32_t t = 0;
@@ -447,12 +339,12 @@ __global__ void __launch_bounds__(WAVE_WARPS * 32) unfilter_wave_kernel(WavePara
         uint32_t*      prev  = band == 0 ? nullptr : p.progress + gidx - 1;
         uint32_t*      mine  = band + 1 < nband ? p.progress + gidx : nullptr;
         switch (job.bpp) {
-        case 1: wave_band<1>(job, band, prev, mine, ring, oring, aring, p.hist); break;
-        case 2: wave_band<2>(job, band, prev, mine, ring, oring, aring, p.hist); break;
-        case 3: wave_band<3>(job, band, prev, mine, ring, oring, aring, p.hist); break;
-        case 4: wave_band<4>(job, band, prev, mine, ring, oring, aring, p.hist); break;
-        case 6: wave_band<6>(job, band, prev, mine, ring, oring, aring, p.hist); break;
-        default: wave_band<8>(job, band, prev, mine, ring, oring, aring, p.hist); break;
+        case 1: wave_band<1>(job, band, prev, mine, ring, p.hist); break;
+        case 2: wave_band<2>(job, band, prev, mine, ring, p.hist); break;
+        case 3: wave_band<3>(job, band, prev, mine, ring, p.hist); break;
+        case 4: wave_band<4>(job, band, prev, mine, ring, p.hist); break;
+        case 6: wave_band<6>(job, band, prev, mine, ring, p.hist); break;
+        default: wave_band<8>(job, band, prev, mine, ring, p.hist); break;
         }
     }
 }

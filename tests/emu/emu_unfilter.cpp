@@ -54,4 +54,3 @@ extern "C" int emu_unfilter_multi(int n, const uint8_t* const* filtered, const u
     simt::launch(grid, WAVE_WARPS * 32, WAVE_SMEM, [&]() { unfilter_wave_kernel(p); }, order, true);
     return 0;
 }
-extern "C" int emu_unfilter_config(int* burst, int* depth, int* warps) { *burst = WAVE_BURST; *depth = WAVE_DEPTH; *warps = WAVE_WARPS; return (int)WAVE_SMEM; }

@@ -1,6 +1,5 @@
-"""unfilter_wave_kernel (csrc/unfilter.cuh) under the host SIMT emulator, in the round-2 configuration (one 16-byte chunk
-per lane and step) and with burst staging (a 128-byte line per row and refill, output collected per line): every filter
-type, ragged widths, misaligned rows, several bands talking through the progress words, against the oracle."""
+"""unfilter_wave_kernel (csrc/unfilter.cuh) under the host SIMT emulator, built exactly as the library builds it: every
+filter type, ragged widths, misaligned rows, several bands talking through the progress words, against the oracle."""
 from __future__ import annotations
 
 import ctypes as C
@@ -18,25 +17,23 @@ from oracle import oracle  # noqa: E402
 HERE = os.path.join(os.path.dirname(__file__), "emu")
 
 
-def build(burst: int, warps: int, extra: tuple = ()):
-    lib = os.path.join(HERE, f"libemu_unfilter_b{burst}w{warps}{'x' * len(extra)}.so")
+def build():
+    lib = os.path.join(HERE, "libemu_unfilter.so")
     src = os.path.join(HERE, "emu_unfilter.cpp")
     dep = os.path.join(HERE, "..", "..", "swift-png_b200", "csrc", "unfilter.cuh")
     if not os.path.exists(lib) or any(os.path.getmtime(d) > os.path.getmtime(lib) for d in (src, dep, os.path.join(HERE, "simt.h"))):
         subprocess.run(["g++", "-O1", "-g", "-std=c++17", "-shared", "-fPIC", "-I" + HERE, "-Wno-attributes",
-                        f"-DPNGB200_WAVE_BURST={burst}", f"-DPNGB200_WAVE_WARPS={warps}", *extra, "-o", lib, src], check=True)
+                        "-o", lib, src], check=True)
     L = C.CDLL(lib)
     L.emu_unfilter.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint, C.c_int]
     return L
 
 
-ABOVE = ("-DPNGB200_WAVE_ABOVE=1", "-DPNGB200_WAVE_LAG=24", "-DPNGB200_WAVE_PUBLISH=16")   # row-above ring + lag hysteresis
-
-
-@pytest.mark.parametrize("burst,warps,extra", [(1, 8, ()), (8, 4, ()), (4, 8, ()), (1, 8, ABOVE)])
-def test_wave_kernel_matches_oracle(burst, warps, extra):
-    L = build(burst, warps, extra)
-    rng = np.random.default_rng(burst * 10 + warps)
+# (scheduling order, CTAs): grid 1 holds 4 warps, fewer than the 7 bands of the 200-row shapes, so warps take later tickets
+@pytest.mark.parametrize("order,grid", [(0, 2), (1, 1), (2, 4), (3, 3)])
+def test_wave_kernel_matches_oracle(order, grid):
+    L = build()
+    rng = np.random.default_rng(14)
     for bpp, depth, w, h in [(4, 8, 300, 100), (4, 8, 37, 70), (8, 16, 129, 67), (3, 8, 211, 40), (1, 8, 1000, 33),
                              (4, 8, 3, 200), (2, 8, 64, 64), (6, 16, 50, 97), (4, 8, 1024, 64)]:
         pitch = w * bpp
@@ -47,18 +44,17 @@ def test_wave_kernel_matches_oracle(burst, warps, extra):
         filtered = rows.tobytes()
         st, want = oracle.png_unfilter(filtered, w, h, 8 * bpp, depth)
         assert st == 0
-        for order, grid in ((0, 2), (3, 3)):
-            src = (C.c_uint8 * (len(filtered) + 64)).from_buffer_copy(filtered + bytes(64))
-            out = (C.c_uint8 * (h * pitch + 64))()
-            L.emu_unfilter(C.addressof(src), len(filtered), C.addressof(out), w, h, bpp, depth, grid, order)
-            assert bytes(out)[: h * pitch] == want, (bpp, depth, w, h, order)
-            assert bytes(out)[h * pitch:] == bytes(64)      # nothing written past the image
+        src = (C.c_uint8 * (len(filtered) + 64)).from_buffer_copy(filtered + bytes(64))
+        out = (C.c_uint8 * (h * pitch + 64))()
+        L.emu_unfilter(C.addressof(src), len(filtered), C.addressof(out), w, h, bpp, depth, grid, order)
+        assert bytes(out)[: h * pitch] == want, (bpp, depth, w, h, order)
+        assert bytes(out)[h * pitch:] == bytes(64)      # nothing written past the image
 
 
 def test_level_major_ticket_order_over_several_images():
     """tickets handed out band level by band level over images of different heights (run_unfilter's order): every band still
     finds the band above it running, every image comes out as the oracle's"""
-    L = build(1, 8)
+    L = build()
     L.emu_unfilter_multi.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
                                      C.c_uint, C.c_int]
     rng = np.random.default_rng(5)
