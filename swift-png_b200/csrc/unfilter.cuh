@@ -13,7 +13,8 @@
 //   the previous row of band k+1, published chunk-by-chunk with a progress counter.  Bands are
 //   handed out by an atomic ticket in row order, so a band's predecessor is always already
 //   running (no deadlock whatever the residency).  Each lane stages its own row through a
-//   shared-memory ring in 16-byte chunks (see WAVE_DEPTH) and writes 16-byte stores.
+//   shared-memory ring in 16-byte chunks (see WAVE_DEPTH) and writes its chunks in pairs: two
+//   back-to-back 16-byte stores that fill a whole 32-byte sector (see wave_band).
 //
 // unfilter_generic_kernel: every other format (Adam7, 1/2/4-bit samples); one CTA per image.
 #pragma once
@@ -130,12 +131,13 @@ struct WaveParams {
 // Asynchronous staging of a lane's own row (cp.async = LDGSTS: global -> shared memory without a register in
 // between).  Every lane keeps a private ring of WAVE_DEPTH aligned 16-byte chunks of its row in shared memory: the
 // first WAVE_DEPTH chunks are issued before the sweep, and step j issues chunk j + WAVE_DEPTH into the slot chunk j
-// has just left.  Reconstructed chunks are stored straight from registers.  The rings are the CTA's whole shared
+// has just left.  Reconstructed chunks are stored from registers, two at a time.  The rings are the CTA's whole shared
 // memory (WAVE_SMEM, 32 KiB); a deeper ring, or a second one for the output or for lane 0's row above, costs resident
 // warps, and the kernel's throughput follows resident warps, not lookahead per warp (DESIGN §4.3).
 constexpr int      WAVE_WARPS   = 4;    // warps per CTA
 constexpr int      WAVE_DEPTH   = 16;   // ring slots per lane
 constexpr int      WAVE_PUBLISH = 8;    // publish progress every this many chunks
+static_assert(WAVE_PUBLISH % 2 == 0, "progress must only ever count chunk pairs that have been stored");
 constexpr unsigned WAVE_POLL_NS = 64;   // lane 0's back-off while the band above has not published the chunk it needs
 constexpr size_t   WAVE_SMEM    = sizeof(uint4) * 32 * (size_t)WAVE_WARPS * WAVE_DEPTH;
 __device__ __forceinline__ void cp_async16(uint4* smem, const uint4* gmem)
@@ -198,6 +200,7 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
 
     uint4    qcur  = make_uint4(0, 0, 0, 0);
     uint4    mine  = make_uint4(0, 0, 0, 0);  // my last reconstructed chunk
+    uint4    held  = make_uint4(0, 0, 0, 0);  // even chunk j, stored together with chunk j + 1
     uint32_t a0 = 0, a1 = 0, c0 = 0, c1 = 0;  // BPP 4/8 histories (words)
     uint64_t ah = 0, ch = 0;                  // generic byte histories
     uint32_t seen = 0;
@@ -289,7 +292,16 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
                 }
                 o = make_uint4(os[0], os[1], os[2], os[3]);
             }
-            store16_partial(out + 16 * (uint64_t)j, o, (int)pitch - 16 * j);
+            // Chunks 2k and 2k + 1 are stored back to back, one step late for the even one: a lone 16-byte store
+            // leaves half a 32-byte sector dirty in L2 for a whole step (thousands of cycles, ~100 K rows in flight),
+            // and on the H100 those half-written sectors cost the kernel half its bandwidth.  The band below reads
+            // this row only up to the published progress, which always counts pairs that have been stored.
+            if ((j & 1) == 0 && j + 1 < nchunk) {
+                held = o;
+            } else {
+                if (j & 1) store16_partial(out + 16 * (uint64_t)(j - 1), held, 16);
+                store16_partial(out + 16 * (uint64_t)j, o, (int)pitch - 16 * j);
+            }
             mine = o;
             if (publish && (((j + 1) % WAVE_PUBLISH) == 0 || j + 1 == nchunk)) {
                 __threadfence();
