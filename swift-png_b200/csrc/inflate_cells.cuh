@@ -45,7 +45,7 @@
 // MRC32 (Sources/LZ77/Wrappers/LZ77.MRC32.swift:26-47).
 #pragma once
 
-#include "inflate_wave.cuh"   // shared pieces: FastBits, wv_decode, wv_fast_header, StagedReader, bulk copy, Adler helpers
+#include "inflate_stream.cuh"   // shared pieces: FastBits, header parsers, bulk copy, Adler-32, stream driver, wave front end
 
 namespace pngb200 {
 
@@ -82,8 +82,8 @@ struct ClShared {
     uint32_t     adler_a[WV_WARPS], adler_b[WV_WARPS];
     uint32_t     exc[WV_WARPS], valid[WV_WARPS];
     uint32_t     last, term, anomaly, ticket;
-    uint32_t     cut_pos, cut_out;
-    uint32_t     hdr_mode, hdr_rel, hdr_ok, hdr_end, hdr_count;   // block header hand-over (see cl_header_preamble)              // a cut wave: bit position of the first token not emitted, bytes emitted
+    uint32_t     cut_pos, cut_out;              // a cut wave: bit position of the first token not emitted, bytes emitted
+    uint32_t     hdr_mode, hdr_rel, hdr_ok, hdr_count;   // block header hand-over (see cl_header_preamble)
     uint64_t     cyc[12], tick;
     uint64_t     pf_bar;
     WvHeader     hdr;
@@ -271,7 +271,7 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
     static_assert(offsetof(ClShared, pf_tail) == offsetof(ClShared, mask) + sizeof(uint32_t) * 8 * WV_THREADS &&
                   sizeof(uint32_t) * WV_PF_WORDS <= sizeof(uint32_t) * (8 * WV_THREADS + 16), "prefetch area = mask ++ pf_tail");
     static_assert(offsetof(ClShared, mask) % 16 == 0 && offsetof(ClShared, cells) % 32 == 0, "alignment");
-    uint32_t pf_parity = 0;
+    WavePrefetch pf{0, false, 0};
     const saddr_t sbase = opaque(smem_addr(cl_smem));
     const saddr_t words_addr = sbase + offsetof(ClShared, words);
     const saddr_t lit = sbase + offsetof(ClShared, ser) + offsetof(SerialShared, lit);
@@ -285,98 +285,34 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
     uint32_t* const tok_mine = tok_own + t * CL_TCAP;
 
     for (;;) {
-        __syncthreads();
-        if (t == 0) {
-            sh.ticket = atomicAdd(P.ticket, 1u);
-            sh.anomaly = 0;
-            for (int k = 0; k < 12; ++k) sh.cyc[k] = 0;
-            sh.tick = (uint64_t)clock64();
-        }
-        __syncthreads();
-        if (sh.ticket >= (uint32_t)P.count) return;
-        const int       j   = P.order ? (int)P.order[sh.ticket] : (int)sh.ticket;
-        const StreamJob job = P.jobs[j];
-        StreamResult*   r   = P.results + j;
-
-        BitReader br;
-        br.init(job.src, job.src_len, job.start_bit);
-        uint64_t out    = job.start_out;
-        uint32_t blocks = 0, waves = 0, sweep_rounds = 0, cuts = 0;
+        const int j = next_stream(sh, P);
+        if (j < 0) return;
+        StreamRun S;
+        S.open(P, j);
+        const StreamJob& job = S.job;
+        StreamResult* const r = S.r;
+        BitReader& br = S.br;
+        uint64_t&  out = S.out;
+        uint32_t waves = 0, sweep_rounds = 0, cuts = 0;
         uint64_t n_tokens = 0, n_matches = 0, walk_tokens = 0;
-        int      st     = PNGB200_OK;
-        uint32_t phase  = (uint32_t)job.phase;
-        uint64_t resume_bit = job.start_bit, resume_out = job.start_out;
         uint8_t* const dst = job.dst;
         const bool     sym = job.symbolic != 0;       // segment: dst is uint16_t[dst_cap]
         uint16_t* const dst16 = reinterpret_cast<uint16_t*>(job.dst);
-        bool fallback = false;
-        bool     pf_pending = false;
-        uint64_t pf_first = 0;
         uint32_t nsub = WV_THREADS;             // subsequences the next wave speculates on
         const bool adler_on = job.start_out == 0 && !sym;
-        uint32_t   s1 = 1, s2 = 0;
-        uint64_t   pend_len = 0;
-        bool       pend = false;
-        auto fold_adler = [&]() {
-            if (pend && t == 0) {
-                uint64_t A = 0, B = 0;
-                for (int w = 0; w < WV_WARPS; ++w) { A += sh.adler_a[w]; B += sh.adler_b[w]; }
-                s2 = (uint32_t)((s2 + (pend_len % ADLER_MOD32) * s1 + B) % ADLER_MOD32);
-                s1 = (uint32_t)((s1 + A) % ADLER_MOD32);
-            }
-            pend = false;
-        };
-        auto adler_hbm = [&](const uint8_t* p, uint64_t n) {
-            uint64_t a = 0, bw = 0;
-            const uint64_t per = (n + WV_THREADS - 1) / WV_THREADS;
-            const uint64_t lo = min((uint64_t)t * per, n), hi = min(lo + per, n);
-            adler_bytes(p + lo, hi - lo, n - lo, a, bw);
-            uint32_t a32 = (uint32_t)(a % ADLER_MOD32), b32 = (uint32_t)(bw % ADLER_MOD32);
-            for (int o = 16; o; o >>= 1) {
-                a32 += __shfl_down_sync(0xffffffffu, a32, o);
-                b32 += __shfl_down_sync(0xffffffffu, b32, o);
-            }
-            if (lane == 0) { sh.adler_a[warp] = a32; sh.adler_b[warp] = b32; }
-            pend = true;
-            pend_len = n;
-        };
-        auto tick = [&](int i) {
-            if (t == 0) {
-                const uint64_t now = (uint64_t)clock64();
-                sh.cyc[i] += now - sh.tick;
-                sh.tick = now;
-            }
-        };
-
-        if (phase == 0) {
-            st = read_stream_header(br, job.format, r);
-            if (st == PNGB200_OK) {
-                resume_bit = br.at();
-                phase = 1;
-            }
-        }
-        if (st == PNGB200_OK && phase == 2) st = read_trailer(br, job.format, r);
-
-        while (st == PNGB200_OK && phase == 1) {
+        AdlerRun   adler;
+        adler.reset();
+        while (S.st == PNGB200_OK && S.phase == 1) {
             __syncthreads();
-            fold_adler();
+            adler.fold(sh);
             {
                 const uint64_t hbase = br.pos >> 5;
-                for (uint32_t k = t; k < WV_HDR_WORDS; k += WV_THREADS) sh.words[k] = br.load_word(hbase + k);
-                __syncthreads();
-                auto slow_header = [&](WvHeader& h) {   // warp 0: the general parser, exact error semantics
-                    int      type0 = 0, final0 = 0, nlit0 = 0, ndist0 = 0;
-                    uint32_t stored0 = 0;
-                    StagedReader sr;
-                    sr.init(sh.words, hbase << 5, br.total_bits, br.pos);
-                    int st0 = parse_block_header(sr, &sh.ser, r, (int)lane, &type0, &final0, &stored0, &nlit0, &ndist0);
-                    h = WvHeader{st0, type0, final0, nlit0, ndist0, stored0, sr.pos};
-                };
+                stage_header_words(sh, br);
                 if (warp == 0) {
                     WvHeader h;
                     uint32_t rel = 0;
                     const int mode = cl_header_preamble(sh, hbase << 5, br.pos, br.total_bits, (int)lane, h, rel);
-                    if (mode == 0) slow_header(h);
+                    if (mode == 0) h = general_block_header(sh, br, r);
                     if (lane == 0) {
                         sh.hdr = h;
                         sh.hdr_mode = (uint32_t)mode;
@@ -437,8 +373,7 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                             for (uint32_t k = 0; k < cnt; ++k) sh.ser.lens[at + k] = (uint8_t)val;
                         }
                     } else if (warp == 0) {
-                        WvHeader h;
-                        slow_header(h);
+                        const WvHeader h = general_block_header(sh, br, r);
                         if (lane == 0) sh.hdr = h;
                     }
 #if defined(PNGB200_EMU) && defined(WV_PROFILE)
@@ -448,28 +383,19 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
             }
             __syncthreads();
             const WvHeader hdr = sh.hdr;
-            st = hdr.status;
-            if (st != PNGB200_OK) break;
+            S.st = hdr.status;
+            if (S.st != PNGB200_OK) break;
             const int      type = hdr.type, final = hdr.final;
             const uint32_t stored = hdr.stored;
             br.seek(hdr.pos);
             if (type != 0) {
-                st = build_block_tables(&sh.ser, r, hdr.nlit, hdr.ndist, (int)t, WV_THREADS);
-                if (st != PNGB200_OK) break;
+                S.st = build_block_tables(&sh.ser, r, hdr.nlit, hdr.ndist, (int)t, WV_THREADS);
+                if (S.st != PNGB200_OK) break;
             }
-            tick(0);
+            phase_tick(sh, 0);
             if (type == 0) {
-                if (!br.have(8 * (uint64_t)stored)) { st = PNGB200_NEED_MORE_INPUT; break; }
-                if (out + stored > job.dst_cap) { st = fail(r, PNGB200_ERR_OUTPUT_CAPACITY); break; }
-                const uint8_t* s = job.src + (br.at() >> 3);
-                if (sym) for (uint32_t k = t; k < stored; k += WV_THREADS) dst16[out + k] = s[k];
-                else for (uint32_t k = t; k < stored; k += WV_THREADS) dst[out + k] = s[k];
-                if (adler_on && stored) adler_hbm(s, stored);
-                out += stored;
-                br.seek(br.pos + 8 * (uint64_t)stored);
-                __syncthreads();
-                fold_adler();
-                tick(9);
+                if (!S.copy_stored(sh, dst, job.dst_cap, sym, stored, adler, adler_on)) break;
+                phase_tick(sh, 9);
             } else {
                 bool block_done = false;
                 while (!block_done) {
@@ -479,27 +405,14 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                     const uint64_t wstart = br.pos;
                     const uint64_t wbase  = (wstart >> 5) & ~(uint64_t)7;
                     __syncthreads();
-                    bool staged = false;
-                    if (pf_pending) {
-                        while (!mbar_try_wait(&sh.pf_bar, pf_parity)) {}
-                        pf_parity ^= 1;
-                        pf_pending = false;
-                        if (wbase >= pf_first && wbase - pf_first < 4) {
-                            const uint32_t* lin = sh.mask + (uint32_t)(wbase - pf_first);
-                            for (uint32_t k = t; k < WV_WORDS; k += WV_THREADS) sh.words[k + (k >> 3)] = lin[k];
-                            staged = true;
-                        }
-                    }
-                    if (!staged)
-                        for (uint32_t k = t; k < WV_WORDS; k += WV_THREADS)
-                            sh.words[k + (k >> 3)] = br.load_word(wbase + k);
+                    pf.stage(sh, br, wbase);
                     if (t == 0) {
                         sh.wcount[0] = 0;
                         sh.cut_pos = 0xffffffffu;
                     }
                     __syncthreads();                                      // (1)
-                    fold_adler();
-                    tick(1);
+                    adler.fold(sh);
+                    phase_tick(sh, 1);
                     const uint32_t rel0  = (uint32_t)(wstart - (wbase << 5));  // < 256
                     const uint32_t base  = t * WV_SUB_BITS;
                     const uint32_t limit = base + WV_SUB_BITS;
@@ -533,7 +446,7 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                     sh.exit_[t] = exit_bit;
                     sh.cross_[t] = 0;
                     __syncthreads();                                      // (2) maps complete
-                    tick(2);
+                    phase_tick(sh, 2);
 
                     // ---- B. walks (as in inflate_wave_kernel) ----
                     {
@@ -606,7 +519,7 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                             }
                         }
                     }
-                    tick(3);
+                    phase_tick(sh, 3);
                     const uint32_t kind = sh.kind_[t], wpos = sh.wpos_[t];
                     {
                         const bool joins_next = kind == WK_SYNC && (wpos >> 8) == t + 1;
@@ -616,38 +529,10 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                     }
                     __syncthreads();                                      // (3)
 
-                    // ---- C. the true chain: orbit of thread 0 ----
-                    if (t == 0) {
-                        uint32_t E[WV_WARPS];
-#pragma unroll
-                        for (int w = 0; w < WV_WARPS; ++w) E[w] = sh.exc[w];
-                        uint32_t cur = 0, x = 0;
-                        bool     done = false;
-#pragma unroll
-                        for (int w = 0; w < WV_WARPS; ++w) {
-                            uint32_t v = 0;
-                            while (!done && cur < 32u * (w + 1)) {
-                                const uint32_t lo = cur - 32u * w;
-                                const uint32_t m = E[w] & (~0u << lo);
-                                if (m == 0) {
-                                    v |= ~0u << lo;
-                                    cur = 32u * (w + 1);
-                                    break;
-                                }
-                                const uint32_t b = (uint32_t)__ffs((int)m) - 1;
-                                x = 32u * w + b;
-                                v |= bit_mask(lo, b + 1);
-                                const uint32_t nx = sh.next_[x];
-                                if (nx == 0xffffu) done = true;
-                                else cur = nx;
-                            }
-                            sh.valid[w] = v;
-                        }
-                        sh.last = x;
-                        sh.term = sh.kind_[x];
-                    }
+                    // ---- C. the true chain ----
+                    if (t == 0) follow_chain(sh);
                     __syncthreads();                                      // (4)
-                    tick(4);
+                    phase_tick(sh, 4);
 
                     // ---- D. my share of the chain ----
                     const bool     on_chain = (sh.valid[warp] >> lane) & 1u;
@@ -731,48 +616,18 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                             kept   = a_hi != 255u && a_hi <= CL_WCAP;
                         }
                     }
-                    const uint64_t mine = (uint64_t)my_ncopy << 40 | my_nout;
-                    uint64_t incl = mine;
-                    for (int o = 1; o < 32; o <<= 1) {
-                        uint64_t v = __shfl_up_sync(0xffffffffu, incl, o);
-                        if ((int)lane >= o) incl += v;
-                    }
-                    if (lane == 31) sh.warp_sums[warp] = incl;
-                    __syncthreads();                                      // (5)
-                    if (warp == 0) {
-                        uint64_t ws = lane < WV_WARPS ? sh.warp_sums[lane] : 0, wi = ws;
-                        for (int o = 1; o < 32; o <<= 1) {
-                            uint64_t v = __shfl_up_sync(0xffffffffu, wi, o);
-                            if ((int)lane >= o) wi += v;
-                        }
-                        if (lane < WV_WARPS) sh.warp_sums[lane] = wi - ws;
-                        if (lane == WV_WARPS - 1) sh.warp_sums[WV_WARPS] = wi;
-                    }
-                    __syncthreads();                                      // (6)
-                    tick(5);
-                    const uint64_t excl    = sh.warp_sums[warp] + incl - mine;
+                    const uint64_t excl    = cta_scan_packed(sh, (uint64_t)my_ncopy << 40 | my_nout);   // (5), (6)
+                    phase_tick(sh, 5);
                     const uint64_t o64     = excl & 0xffffffffffull;
                     const uint64_t total64 = sh.warp_sums[WV_WARPS] & 0xffffffffffull;
                     const uint32_t np      = (uint32_t)(sh.warp_sums[WV_WARPS] >> 40);
                     const bool     cut     = total64 > CL_CAP;            // the wave is cut at the token that would overflow the cells
                     if (sh.anomaly || out + total64 > job.dst_cap) {
-                        fallback = true;
+                        S.fallback = true;
                         break;
                     }
                     // ---- prefetch of the next wave's words (predicted start; a cut wave misses and stages directly) ----
-                    if (!cut) {
-                        const uint64_t nbase = wbase + wave_bits / 32;
-                        const uint64_t first = nbase - ((((uintptr_t)br.words >> 2) + nbase) & 3);
-                        if (first >= 1 && (first + WV_PF_WORDS + 1) * 32 <= br.total_bits) {
-                            if (t == 0) {
-                                fence_proxy_async();
-                                mbar_expect_tx(&sh.pf_bar, sizeof(uint32_t) * WV_PF_WORDS);
-                                bulk_g2s(sh.mask, br.words + first, sizeof(uint32_t) * WV_PF_WORDS, &sh.pf_bar);
-                            }
-                            pf_pending = true;
-                            pf_first = first;
-                        }
-                    }
+                    if (!cut) pf.start(sh, br, wbase + wave_bits / 32);
                     // ---- E. emit: decode my share once more, write cells ----
                     uint8_t* const wdst  = dst + (sym ? 2 * out : out);      // HBM address of wave offset 0
                     // slot of wave offset 0: dst's phase inside a 16-element store unit (16 bytes, or 16 symbols = 32 bytes)
@@ -843,9 +698,9 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                     WV_COUNT(3, from_staging);
                     if (cut && my_stop != 0xffffffffu) atomicMin(&sh.cut_pos, my_stop);
                     __syncthreads();                                      // (7) cells written
-                    tick(6);
+                    phase_tick(sh, 6);
                     if (sh.anomaly) {
-                        fallback = true;
+                        S.fallback = true;
                         break;
                     }
                     uint32_t total = (uint32_t)total64;
@@ -898,7 +753,7 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                         sweep_rounds += rounds;
                         WV_COUNT(4, rounds);
                     }
-                    tick(7);
+                    phase_tick(sh, 7);
                     // ---- G (segment). store: cells -> 16-bit symbols; a window cell takes the symbol stored at that position
                     //      (byte or marker), or becomes a marker when the position lies in front of the segment ----
                     if (sym && total) {
@@ -985,18 +840,9 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                                 bw += (end - k) * v;
                             }
                         }
-                        if (adler_on) {
-                            uint32_t a32 = a, b32 = bw % ADLER_MOD32;
-                            for (int o2 = 16; o2; o2 >>= 1) {
-                                a32 += __shfl_down_sync(0xffffffffu, a32, o2);
-                                b32 += __shfl_down_sync(0xffffffffu, b32, o2);
-                            }
-                            if (lane == 0) { sh.adler_a[warp] = a32; sh.adler_b[warp] = b32; }
-                            pend = true;
-                            pend_len = total;
-                        }
+                        if (adler_on) adler.piece_from_partials(sh, a, bw % ADLER_MOD32, total);
                     }
-                    tick(8);
+                    phase_tick(sh, 8);
                     out += total;
                     if (t == 0) n_matches += np;
                     n_tokens += emitted;
@@ -1013,88 +859,14 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                         if (term == WK_EOB || term == WK_OWN_EOB) block_done = true;
                     }
                 }
-                if (fallback) break;
+                if (S.fallback) break;
             }
-            ++blocks;
-            resume_bit = br.at();
-            resume_out = out;
-            if (job.stop_bit && !final && br.at() >= job.stop_bit) break;   // end of my segment (the host checks ==)
-            if (final) {
-                phase = 2;
-                st = read_trailer(br, job.format, r);
-                break;
-            }
+            if (S.end_block(final)) break;
         }
-        if (pf_pending) {
-            while (!mbar_try_wait(&sh.pf_bar, pf_parity)) {}
-            pf_parity ^= 1;
-            pf_pending = false;
-        }
-        __syncthreads();
-        fold_adler();
-        __syncthreads();   // thread 0 has read the last piece's sums before the statistics reuse sh.adler_b
-        {
-            uint64_t v0 = n_tokens, v2 = walk_tokens;
-            uint32_t v3 = sweep_rounds;
-            for (int o = 16; o; o >>= 1) {
-                v0 += __shfl_down_sync(0xffffffffu, v0, o);
-                v2 += __shfl_down_sync(0xffffffffu, v2, o);
-                v3 = max(v3, __shfl_down_sync(0xffffffffu, v3, o));
-            }
-            if (lane == 0) {
-                sh.warp_sums[warp] = v0;
-                sh.adler_b[warp] = (uint32_t)min(v2, (uint64_t)0xffffffffu);
-                sh.exc[warp] = v3;
-            }
-            __syncthreads();
-            if (t == 0) {
-                uint64_t tk = 0, wt = 0;
-                uint32_t rr = 0;
-                for (int w = 0; w < WV_WARPS; ++w) {
-                    tk += sh.warp_sums[w];
-                    wt += sh.adler_b[w];
-                    rr = max(rr, sh.exc[w]);
-                }
-                r->stat_waves          = waves;
-                r->stat_sync_rounds    = (uint32_t)min(wt, (uint64_t)0xffffffffu);   // tokens decoded by walks
-                r->stat_resolve_rounds = rr;                                          // pointer-jumping rounds
-                r->stat_tokens         = tk;
-                r->stat_matches        = n_matches;
-                r->stat_deferred       = cuts;                                        // waves cut at the cell capacity
-                for (int k = 0; k < 12; ++k) r->stat_cycles[k] = sh.cyc[k];
-            }
-        }
-        if (fallback && sym) {
-            // a segment cannot go through the byte-wise serial decoder: report it, the host decodes the stream whole
-            if (t == 0) {
-                r->status = PNGB200_ERR_INTERNAL;
-                r->produced = out;
-                r->consumed_bits = br.at();
-                r->blocks = blocks;
-            }
-        } else if (fallback) {
-            __syncthreads();
-            if (warp == 0) serial_inflate(sh.ser, job, r, resume_bit, resume_out, 1, blocks);
-        } else if (t == 0) {
-            if (r->status == 0) r->status = st;
-            r->produced      = out;
-            r->consumed_bits = br.at();
-            r->blocks        = blocks;
-            r->resume_bit    = resume_bit;
-            r->resume_out    = resume_out;
-            r->phase         = phase;
-            if (adler_on && job.format != PNGB200_FORMAT_GZIP) {
-                const uint32_t computed = s2 << 16 | s1;
-                r->checksum = computed;
-                r->ck_done  = 1;
-                if (r->trailer_seen && job.format != PNGB200_FORMAT_IOS && r->status >= 0 && r->declared != computed) {
-                    r->status = PNGB200_ERR_STREAM_CHECKSUM;
-                    r->err_a  = r->declared;
-                    r->err_b  = computed;
-                }
-            }
-        }
-        if (t == 0) r->stat_fallback = fallback ? 1u : 0u;
+        pf.drain(sh);
+        // stat_deferred: waves cut at the cell capacity; stat_resolve_rounds: pointer-jumping rounds
+        S.finish(sh, adler, adler_on, PNGB200_ERR_INTERNAL,
+                 [&] { report_wave_stats(sh, r, waves, n_matches, n_tokens, t == 0 ? cuts : 0, walk_tokens, sweep_rounds); });
     }
 }
 

@@ -36,7 +36,7 @@
 // (Sources/LZ77/Inflator/LZ77.InflatorBuffers.Stream.swift:266-381, LZ77.InflatorOut.swift:124-140).
 #pragma once
 
-#include "inflate_wave.cuh"   // shared pieces: FastBits, fast_lookup, StagedReader, wv_fast_header, CopyItem
+#include "inflate_stream.cuh"   // shared pieces: FastBits, fast_lookup, header parsers, CopyItem, Adler-32, CTA scan
 
 namespace pngb200 {
 namespace par {
@@ -52,13 +52,7 @@ constexpr uint32_t PAR_SMEM_WORDS   = PAR_WAVE_WORDS + PAR_WAVE_WORDS / 8 + 1;
 constexpr uint32_t PAR_OUT_BYTES    = 16384;                         // wave output image in smem
 constexpr uint32_t PAR_BITMAP_WORDS = PAR_OUT_BYTES / 32;
 constexpr uint32_t PAR_LIST_CAP     = PAR_THREADS * (PAR_SUB_BITS / 2);  // >= copies per wave (2 bits min each)
-constexpr uint64_t PAR_MAX_WAVE_OUT = (uint64_t)PAR_LIST_CAP * 258;
-
-struct ParHeader {  // block header as parsed by warp 0, broadcast to the CTA
-    int32_t  status, type, final, nlit, ndist;
-    uint32_t stored;
-    uint64_t pos;     // reader position after the header
-};
+static_assert(PAR_THREADS == WV_THREADS, "the stream driver (inflate_stream.cuh) works in CTAs of WV_THREADS");
 
 struct ParShared {
     SerialShared ser;
@@ -75,24 +69,14 @@ struct ParShared {
     uint32_t     first_need[2], first_stop[2], nlist[2];
     uint32_t     npend, anomaly, ticket, pad;
     uint64_t     cyc[12], tick;         // phase timers (thread 0), as in inflate_wave_kernel
-    // running Adler-32 of the stream (zlib / ios streams decoded from their first byte), folded wave by wave from the
-    // partial sums the store phase leaves here: no second pass over the inflated bytes (as in inflate_wave_kernel)
-    uint64_t     pend_len;
-    uint32_t     s1, s2, pend;
+    // running Adler-32 of the stream (zlib / ios streams decoded from their first byte): in shared memory here, where
+    // registers are short
+    AdlerRun     adler;
     uint32_t     adler_a[PAR_WARPS], adler_b[PAR_WARPS];
-    ParHeader    hdr;
+    WvHeader     hdr;
 };
 
-struct ParParams {
-    const StreamJob* jobs;
-    StreamResult*    results;
-    const uint32_t*  order;
-    uint32_t*        ticket;       // global work counter (zeroed before launch)
-    uint8_t*         scratch;      // per-CTA: copy list + unresolved bitmap for oversized waves
-    uint64_t         scratch_stride;
-    uint64_t         bitmap_words; // size of the HBM bitmap of each CTA
-    int              count;
-};
+using ParParams = WvParams;   // the round-1 kernels take the ring kernel's parameter block
 
 // sync-phase decode: symbol boundaries and output byte count only
 __device__ __forceinline__ void par_decode_count(const ParShared& sh, uint32_t start, uint32_t limit,
@@ -206,7 +190,7 @@ __device__ __forceinline__ void lz_copy(uint8_t* img, const uint8_t* hbm, bool i
 
 // One body, two register budgets: 4 CTAs per SM (64 registers, a few spills) when there are streams for them, 3 CTAs
 // per SM (80 registers, none) when the batch only fills three slots per SM anyway -- the 444 x 8K benchmark batch.
-__device__ __forceinline__ void inflate_parallel_body(ParParams P)
+__device__ __forceinline__ void inflate_parallel_body(WvParams P)
 {
     PNGB200_DYN_SMEM(par_smem);
     ParShared& sh = *reinterpret_cast<ParShared*>(par_smem);
@@ -218,40 +202,9 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
     for (uint32_t k = t; k < PAR_BITMAP_WORDS; k += PAR_THREADS) sh.bitmap[k] = 0;
 
     for (;;) {
-        __syncthreads();
-        if (t == 0) {
-            sh.ticket = atomicAdd(P.ticket, 1u);
-            sh.anomaly = 0;
-            for (int k = 0; k < 12; ++k) sh.cyc[k] = 0;
-            sh.tick = (uint64_t)clock64();
-            sh.s1 = 1;
-            sh.s2 = 0;
-            sh.pend = 0;
-        }
-// fold the partial sums of the piece that was stored last into (s1, s2); call right after a barrier
-#define PAR_FOLD_ADLER()                                                                                     \
-    do {                                                                                                     \
-        if (t == 0 && sh.pend) {                                                                             \
-            uint64_t A_ = 0, B_ = 0;                                                                         \
-            for (int w_ = 0; w_ < PAR_WARPS; ++w_) { A_ += sh.adler_a[w_]; B_ += sh.adler_b[w_]; }           \
-            sh.s2 = (uint32_t)((sh.s2 + (sh.pend_len % ADLER_MOD32) * sh.s1 + B_) % ADLER_MOD32);            \
-            sh.s1 = (uint32_t)((sh.s1 + A_) % ADLER_MOD32);                                                  \
-            sh.pend = 0;                                                                                     \
-        }                                                                                                    \
-    } while (0)
-// thread 0 charges the cycles since the last tick to phase i: 0 header+tables, 1 stage, 3 speculate + re-decode
-// rounds, 5 scan, 6 emit, 7 resolve, 8 store
-#define PAR_TICK(i)                                          \
-    do {                                                     \
-        if (t == 0) {                                        \
-            const uint64_t now_ = (uint64_t)clock64();       \
-            sh.cyc[i] += now_ - sh.tick;                     \
-            sh.tick = now_;                                  \
-        }                                                    \
-    } while (0)
-        __syncthreads();
-        if (sh.ticket >= (uint32_t)P.count) return;
-        const int       j   = P.order ? (int)P.order[sh.ticket] : (int)sh.ticket;
+        const int j = next_stream(sh, P);
+        if (j < 0) return;
+        if (t == 0) sh.adler.reset();
         const StreamJob job = P.jobs[j];
         StreamResult*   r   = P.results + j;
 
@@ -265,21 +218,6 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
         uint8_t* const dst = job.dst;
         bool fallback = false;
         const bool adler_on = job.start_out == 0;   // this launch sees the stream from its first byte
-        // CTA-wide partial sums of `n` finished bytes at HBM address `p` (stored blocks, oversized waves)
-        auto adler_hbm = [&](const uint8_t* p, uint64_t n) {
-            uint64_t a = 0, bw = 0;
-            const uint64_t per = (n + PAR_THREADS - 1) / PAR_THREADS;
-            const uint64_t lo = min((uint64_t)t * per, n), hi = min(lo + per, n);
-            adler_bytes(p + lo, hi - lo, n - lo, a, bw);
-            uint32_t a32 = (uint32_t)(a % ADLER_MOD32), b32 = (uint32_t)(bw % ADLER_MOD32);
-            for (int o = 16; o; o >>= 1) {
-                a32 += __shfl_down_sync(0xffffffffu, a32, o);
-                b32 += __shfl_down_sync(0xffffffffu, b32, o);
-            }
-            if (lane == 0) { sh.adler_a[warp] = a32; sh.adler_b[warp] = b32; }
-            if (t == 0) { sh.pend = 1; sh.pend_len = n; }
-        };
-
         if (phase == 0) {
             st = read_stream_header(br, job.format, r);
             if (st == PNGB200_OK) {
@@ -290,28 +228,9 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
         if (st == PNGB200_OK && phase == 2) st = read_trailer(br, job.format, r);
 
         while (st == PNGB200_OK && phase == 1) {
-            // warp 0 walks the header bits alone; the CTA then builds the tables together
             __syncthreads();
-            PAR_FOLD_ADLER();
-            {
-                const uint64_t hbase = br.pos >> 5;
-                for (uint32_t k = t; k < WV_HDR_WORDS; k += PAR_THREADS) sh.words[k] = br.load_word(hbase + k);
-                __syncthreads();
-                if (warp == 0) {
-                    WvHeader h;
-                    if (!wv_fast_header(sh, hbase << 5, br.pos, br.total_bits, (int)lane, h)) {
-                        int      type0 = 0, final0 = 0, nlit0 = 0, ndist0 = 0;
-                        uint32_t stored0 = 0;
-                        StagedReader sr;
-                        sr.init(sh.words, hbase << 5, br.total_bits, br.pos);
-                        int st0 = parse_block_header(sr, &sh.ser, r, (int)lane, &type0, &final0, &stored0, &nlit0, &ndist0);
-                        h = WvHeader{st0, type0, final0, nlit0, ndist0, stored0, sr.pos};
-                    }
-                    if (lane == 0) sh.hdr = ParHeader{h.status, h.type, h.final, h.nlit, h.ndist, h.stored, h.pos};
-                }
-            }
-            __syncthreads();
-            const ParHeader hdr = sh.hdr;
+            sh.adler.fold(sh);
+            const WvHeader hdr = read_block_header(sh, br, r);
             st = hdr.status;
             if (st != PNGB200_OK) break;
             const int      type = hdr.type, final = hdr.final;
@@ -321,17 +240,17 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
                 st = build_block_tables(&sh.ser, r, hdr.nlit, hdr.ndist, (int)t, PAR_THREADS);
                 if (st != PNGB200_OK) break;
             }
-            PAR_TICK(0);
+            phase_tick(sh, 0);
             if (type == 0) {
                 if (!br.have(8 * (uint64_t)stored)) { st = PNGB200_NEED_MORE_INPUT; break; }
                 if (out + stored > job.dst_cap) { st = fail(r, PNGB200_ERR_OUTPUT_CAPACITY); break; }
                 const uint8_t* s = job.src + (br.at() >> 3);
                 for (uint32_t k = t; k < stored; k += PAR_THREADS) dst[out + k] = s[k];
-                if (adler_on && stored) adler_hbm(s, stored);
+                if (adler_on && stored) sh.adler.piece_from_hbm(sh, s, stored);
                 out += stored;
                 br.seek(br.pos + 8 * (uint64_t)stored);
                 __syncthreads();
-                PAR_FOLD_ADLER();
+                sh.adler.fold(sh);
             } else {
                 bool block_done = false;
                 while (!block_done) {
@@ -340,7 +259,7 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
                     const uint64_t wstart = br.pos;                       // absolute bit (reader space)
                     const uint64_t wbase  = (wstart >> 5) & ~(uint64_t)7; // first staged word
                     __syncthreads();
-                    PAR_FOLD_ADLER();
+                    sh.adler.fold(sh);
                     for (uint32_t k = t; k < PAR_WAVE_WORDS; k += PAR_THREADS)
                         sh.words[k + (k >> 3)] = br.load_word(wbase + k);
                     if (t == 0) {
@@ -350,7 +269,7 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
                         sh.nlist[0] = sh.nlist[1] = 0;
                     }
                     __syncthreads();
-                    PAR_TICK(1);
+                    phase_tick(sh, 1);
                     const uint32_t rel0  = (uint32_t)(wstart - (wbase << 5));  // < 256
                     const uint32_t limit = (t + 1) * PAR_SUB_BITS;
                     {
@@ -407,32 +326,14 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
                         }
                     }
                     __syncthreads();
-                    PAR_TICK(3);
+                    phase_tick(sh, 3);
                     const uint32_t my_start = sh.start_[t], n = sh.nout_[t];
                     // ---- anomalies on the verified chain -> serial decoder ----
                     if (t == nvalid - 1 && ((sh.flag_[t] & PF_BAD) || (wbase << 5) + sh.exit_[t] > br.total_bits))
                         sh.anomaly = 1;
-                    // ---- scan of output byte counts and copy counts (packed: copies << 40 | bytes) ----
-                    const uint64_t mine = t < nvalid ? ((uint64_t)sh.ncopy_[t] << 40 | n) : 0;
-                    uint64_t incl = mine;
-                    for (int o = 1; o < 32; o <<= 1) {
-                        uint64_t v = __shfl_up_sync(0xffffffffu, incl, o);
-                        if ((int)lane >= o) incl += v;
-                    }
-                    if (lane == 31) sh.warp_sums[warp] = incl;
-                    __syncthreads();
-                    if (warp == 0) {
-                        uint64_t ws = lane < PAR_WARPS ? sh.warp_sums[lane] : 0, wi = ws;
-                        for (int o = 1; o < 32; o <<= 1) {
-                            uint64_t v = __shfl_up_sync(0xffffffffu, wi, o);
-                            if ((int)lane >= o) wi += v;
-                        }
-                        if (lane < PAR_WARPS) sh.warp_sums[lane] = wi - ws;  // exclusive
-                        if (lane == PAR_WARPS - 1) sh.warp_sums[PAR_WARPS] = wi;  // wave totals
-                    }
-                    __syncthreads();
-                    PAR_TICK(5);
-                    const uint64_t excl    = sh.warp_sums[warp] + incl - mine;
+                    // ---- scan of output byte counts and copy counts ----
+                    const uint64_t excl    = cta_scan_packed(sh, t < nvalid ? ((uint64_t)sh.ncopy_[t] << 40 | n) : 0);
+                    phase_tick(sh, 5);
                     const uint32_t o_start = (uint32_t)(excl & 0xffffffffffull);
                     uint32_t       c_next  = (uint32_t)(excl >> 40);           // my first list slot
                     const uint32_t total   = (uint32_t)(sh.warp_sums[PAR_WARPS] & 0xffffffffffull);
@@ -502,7 +403,7 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
                     }
                     __threadfence_block();
                     __syncthreads();
-                    PAR_TICK(6);
+                    phase_tick(sh, 6);
                     // ---- resolve: no CTA barriers.  The list is sorted by output offset and a copy only
                     //      depends on smaller offsets, so a lane may simply block on its current item
                     //      (items t, t + 512, ... in order): the smallest open item is always ready ----
@@ -549,7 +450,7 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
                     }
                     __threadfence_block();
                     __syncthreads();
-                    PAR_TICK(7);
+                    phase_tick(sh, 7);
                     if (sh.anomaly) {
                         // leave the bitmap clean for whoever uses it next
                         for (uint32_t k = t; k < (total + 31) / 32; k += PAR_THREADS) U[k] = 0;
@@ -578,19 +479,11 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
                                 }
                             }
                         }
-                        if (adler_on) {
-                            uint32_t a32 = a, b32 = bw % ADLER_MOD32;
-                            for (int o = 16; o; o >>= 1) {
-                                a32 += __shfl_down_sync(0xffffffffu, a32, o);
-                                b32 += __shfl_down_sync(0xffffffffu, b32, o);
-                            }
-                            if (lane == 0) { sh.adler_a[warp] = a32; sh.adler_b[warp] = b32; }
-                            if (t == 0) { sh.pend = 1; sh.pend_len = total; }
-                        }
+                        if (adler_on) sh.adler.piece_from_partials(sh, a, bw % ADLER_MOD32, total);
                     } else if (in_hbm && adler_on && total) {
-                        adler_hbm(wdst, total);
+                        sh.adler.piece_from_hbm(sh, wdst, total);
                     }
-                    PAR_TICK(8);
+                    phase_tick(sh, 8);
                     out += total;
                     br.seek((wbase << 5) + sh.exit_[nvalid - 1]);
                     if (stop_found) block_done = true;
@@ -607,7 +500,7 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
             }
         }
         __syncthreads();
-        PAR_FOLD_ADLER();
+        sh.adler.fold(sh);
         if (fallback) {
             // the serial decoder redoes this block (and whatever follows) and owns the result record
             __syncthreads();
@@ -620,17 +513,7 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
             r->resume_bit    = resume_bit;
             r->resume_out    = resume_out;
             r->phase         = phase;
-            if (adler_on && job.format != PNGB200_FORMAT_GZIP) {
-                // LZ77.InflatorBuffers.advance(.checksum): compare with the trailer (InflatorBuffers.swift:109-130)
-                const uint32_t computed = sh.s2 << 16 | sh.s1;
-                r->checksum = computed;
-                r->ck_done  = 1;
-                if (r->trailer_seen && job.format != PNGB200_FORMAT_IOS && r->status >= 0 && r->declared != computed) {
-                    r->status = PNGB200_ERR_STREAM_CHECKSUM;
-                    r->err_a  = r->declared;
-                    r->err_b  = computed;
-                }
-            }
+            if (adler_on) sh.adler.check_trailer(r, job.format);
         }
         if (t == 0) {
             for (int k = 0; k < 12; ++k) r->stat_cycles[k] = sh.cyc[k];
@@ -642,8 +525,8 @@ __device__ __forceinline__ void inflate_parallel_body(ParParams P)
     }
 }
 
-__global__ void __launch_bounds__(PAR_THREADS, PAR_CTAS_PER_SM) inflate_parallel_kernel(ParParams P) { inflate_parallel_body(P); }
-__global__ void __launch_bounds__(PAR_THREADS, 3) inflate_parallel_kernel3(ParParams P) { inflate_parallel_body(P); }
+__global__ void __launch_bounds__(PAR_THREADS, PAR_CTAS_PER_SM) inflate_parallel_kernel(WvParams P) { inflate_parallel_body(P); }
+__global__ void __launch_bounds__(PAR_THREADS, 3) inflate_parallel_kernel3(WvParams P) { inflate_parallel_body(P); }
 
 #ifndef PNGB200_EMU
 // host side: opt in to the large dynamic shared memory on the current device (once per context)
@@ -656,16 +539,9 @@ inline int configure_inflate_parallel()
 }
 #endif
 
-inline uint64_t par_bitmap_words(uint64_t max_dst_cap)
-{
-    uint64_t bytes = max_dst_cap < PAR_MAX_WAVE_OUT ? max_dst_cap : PAR_MAX_WAVE_OUT;
-    return (bytes + 31) / 32 + 8;
-}
-inline uint64_t par_scratch_stride(uint64_t bitmap_words)
-{
-    uint64_t s = sizeof(CopyItem) * (uint64_t)PAR_LIST_CAP + 4 * bitmap_words;
-    return (s + 255) / 256 * 256;
-}
+// per-CTA HBM scratch of the round-1 kernels (see wave_bitmap_words)
+inline uint64_t par_bitmap_words(uint64_t max_dst_cap) { return wave_bitmap_words(max_dst_cap, PAR_LIST_CAP); }
+inline uint64_t par_scratch_stride(uint64_t bitmap_words) { return wave_scratch_stride(bitmap_words, PAR_LIST_CAP); }
 
 }  // namespace par
 using par::ParParams;

@@ -18,7 +18,7 @@
 #pragma once
 
 #include "common.cuh"
-#include "inflate_wave.cuh"
+#include "inflate_stream.cuh"   // shared pieces: Adler-32 helpers
 
 namespace pngb200 {
 

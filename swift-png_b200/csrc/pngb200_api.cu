@@ -217,30 +217,15 @@ int launch_waves(pngb200_ctx* ctx, Engine engine, const StreamJob* jobs, StreamR
     CU(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), ctx->stream));
     if (before_launch)
         if (int rc = before_launch()) return rc;
-    auto fill = [&](auto& pp) {
-        pp.jobs = jobs;
-        pp.results = results;
-        pp.order = order;
-        pp.ticket = ticket;
-        pp.scratch = ctx->d_scratch.as<uint8_t>();
-        pp.scratch_stride = stride;
-        pp.bitmap_words = bitmap_words;
-        pp.count = (int)count;
-    };
-    if (engine == ENG_PARALLEL) {
-        ParParams pp{};
-        fill(pp);
-        if (count <= (size_t)ctx->sm_count * 3)
-            inflate_parallel_kernel3<<<grid, PAR_THREADS, sizeof(ParShared), ctx->stream>>>(pp);
-        else
-            inflate_parallel_kernel<<<grid, PAR_THREADS, sizeof(ParShared), ctx->stream>>>(pp);
-    } else {
-        WvParams pp{};
-        fill(pp);
-        pp.switched = switched;
-        if (engine == ENG_CELLS) inflate_cells_kernel<<<grid, WV_THREADS, sizeof(ClShared), ctx->stream>>>(pp);
-        else inflate_wave_kernel<<<grid, WV_THREADS, sizeof(WvShared), ctx->stream>>>(pp);
-    }
+    const WvParams pp{jobs, results, order, ticket, ctx->d_scratch.as<uint8_t>(), stride, bitmap_words, (int)count, switched};
+    if (engine == ENG_PARALLEL && count <= (size_t)ctx->sm_count * 3)
+        inflate_parallel_kernel3<<<grid, PAR_THREADS, sizeof(ParShared), ctx->stream>>>(pp);
+    else if (engine == ENG_PARALLEL)
+        inflate_parallel_kernel<<<grid, PAR_THREADS, sizeof(ParShared), ctx->stream>>>(pp);
+    else if (engine == ENG_CELLS)
+        inflate_cells_kernel<<<grid, WV_THREADS, sizeof(ClShared), ctx->stream>>>(pp);
+    else
+        inflate_wave_kernel<<<grid, WV_THREADS, sizeof(WvShared), ctx->stream>>>(pp);
     ctx->launches++;
     return PNGB200_OK;
 }
