@@ -870,12 +870,4 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
     }
 }
 
-#ifndef PNGB200_EMU
-inline int configure_inflate_cells()
-{
-    return (int)cudaFuncSetAttribute(inflate_cells_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)sizeof(ClShared));
-}
-#endif
-
 }  // namespace pngb200

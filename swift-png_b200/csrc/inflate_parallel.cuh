@@ -528,17 +528,6 @@ __device__ __forceinline__ void inflate_parallel_body(WvParams P)
 __global__ void __launch_bounds__(PAR_THREADS, PAR_CTAS_PER_SM) inflate_parallel_kernel(WvParams P) { inflate_parallel_body(P); }
 __global__ void __launch_bounds__(PAR_THREADS, 3) inflate_parallel_kernel3(WvParams P) { inflate_parallel_body(P); }
 
-#ifndef PNGB200_EMU
-// host side: opt in to the large dynamic shared memory on the current device (once per context)
-inline int configure_inflate_parallel()
-{
-    int rc = (int)cudaFuncSetAttribute(inflate_parallel_kernel3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ParShared));
-    if (rc) return rc;
-    return (int)cudaFuncSetAttribute(inflate_parallel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)sizeof(ParShared));
-}
-#endif
-
 // per-CTA HBM scratch of the round-1 kernels (see wave_bitmap_words)
 inline uint64_t par_bitmap_words(uint64_t max_dst_cap) { return wave_bitmap_words(max_dst_cap, PAR_LIST_CAP); }
 inline uint64_t par_scratch_stride(uint64_t bitmap_words) { return wave_scratch_stride(bitmap_words, PAR_LIST_CAP); }
@@ -552,7 +541,4 @@ using par::PAR_THREADS;
 using par::PAR_CTAS_PER_SM;
 using par::par_bitmap_words;
 using par::par_scratch_stride;
-#ifndef PNGB200_EMU
-using par::configure_inflate_parallel;
-#endif
 }  // namespace pngb200

@@ -756,15 +756,6 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
     }
 }
 
-#ifndef PNGB200_EMU
-// host side: opt in to the large dynamic shared memory on the current device (once per context)
-inline int configure_inflate_wave()
-{
-    return (int)cudaFuncSetAttribute(inflate_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)sizeof(WvShared));
-}
-#endif
-
 // per-CTA HBM scratch of inflate_wave_kernel (see wave_bitmap_words)
 inline uint64_t wv_bitmap_words(uint64_t max_dst_cap) { return wave_bitmap_words(max_dst_cap, WV_LIST_CAP); }
 inline uint64_t wv_scratch_stride(uint64_t bitmap_words) { return wave_scratch_stride(bitmap_words, WV_LIST_CAP); }

@@ -62,8 +62,6 @@ struct FileWalk {
     size_t   first_idat = (size_t)-1, idat_end = 0;  // [first_idat, idat_end): the contiguous IDAT run
 };
 
-inline int channels_of_color(int color) { return color == 0 || color == 3 ? 1 : color == 2 ? 3 : color == 4 ? 2 : 4; }
-
 // Walks the chunk headers of one file and parses IHDR / PLTE / tRNS into `d`
 // (PNG.Image.decompress(stream:), PNG.Image.swift:298-401; PNG.Header.init(parsing:standard:),
 // Parsing/PNG.Header.swift:40-98; PNG.Palette.init(parsing:pixel:), PNG.Palette.swift:27-55;
@@ -112,15 +110,9 @@ void walk_file(pngb200_png_desc& d, FileWalk& w)
         const uint8_t* h = f + c.off + 8;
         if (c.len != 13) return stop(PNGB200_ERR_PARSE_HEADER_CHUNK_LENGTH, c.len, 0, false);
         const int depth = h[8], color = h[9];
-        bool ok;  // PNG.Format.Pixel.recognize(code:)
-        switch (color) {
-        case 0: ok = depth == 1 || depth == 2 || depth == 4 || depth == 8 || depth == 16; break;
-        case 3: ok = depth == 1 || depth == 2 || depth == 4 || depth == 8; break;
-        case 2: case 4: case 6: ok = depth == 8 || depth == 16; break;
-        default: ok = false;
-        }
-        if (!ok) return stop(PNGB200_ERR_PARSE_HEADER_PIXEL_FORMAT_CODE, (uint32_t)depth, (uint32_t)color, false);
-        if (d.standard == 1 && !(depth == 8 && (color == 2 || color == 6)))
+        const PixelRule rule = pixel_rule(color, depth, false);
+        if (!rule.valid) return stop(PNGB200_ERR_PARSE_HEADER_PIXEL_FORMAT_CODE, (uint32_t)depth, (uint32_t)color, false);
+        if (d.standard == 1 && !pixel_rule(color, depth, true).valid)
             return stop(PNGB200_ERR_PARSE_HEADER_PIXEL_FORMAT, (uint32_t)depth, (uint32_t)color, false);
         if (h[10]) return stop(PNGB200_ERR_PARSE_HEADER_COMPRESSION_CODE, h[10], 0, false);
         if (h[11]) return stop(PNGB200_ERR_PARSE_HEADER_FILTER_CODE, h[11], 0, false);
@@ -129,7 +121,7 @@ void walk_file(pngb200_png_desc& d, FileWalk& w)
         if (!d.width || !d.height) return stop(PNGB200_ERR_PARSE_HEADER_SIZE, d.width, d.height, false);
         {
             // the reference traps when the storage size overflows (PNG.Image.swift:84); refuse such a file here
-            const uint64_t bpp = (uint64_t)((depth * channels_of_color(color) + 7) >> 3);
+            const uint64_t bpp = (uint64_t)((depth * rule.channels + 7) >> 3);
             uint64_t prod;
             if (d.width > 0x7fffffffu || d.height > 0x7fffffffu ||
                 __builtin_mul_overflow((uint64_t)d.width * d.height, bpp ? bpp : 1, &prod) || prod > (1ull << 46))
@@ -137,7 +129,7 @@ void walk_file(pngb200_png_desc& d, FileWalk& w)
         }
         d.depth = (uint8_t)depth, d.color = (uint8_t)color, d.interlaced = h[12];
         d.format.color = d.color, d.format.depth = d.depth, d.format.bgr = d.standard;
-        d.storage_size = (uint64_t)d.width * d.height * (uint64_t)((depth * channels_of_color(color) + 7) >> 3);
+        d.storage_size = (uint64_t)d.width * d.height * (uint64_t)((depth * rule.channels + 7) >> 3);
     }
     bool     have_palette = false, have_background = false, have_transparency = false;
     uint32_t npal = 0, nalpha = 0;
@@ -226,6 +218,20 @@ struct CrcPlan {
     size_t    acc_bytes = 0, off_acc = 0;
     bool      any = false;
 };
+// The first piece of each item (CrcRegion or CopySegment: CRC_PIECE bytes a piece, at least one per item), then the
+// total, in `base`; false when the pieces do not fit a launch
+template <typename Item>
+bool piece_bases(const std::vector<Item>& items, std::vector<uint32_t>& base)
+{
+    base.resize(items.size() + 1);
+    uint64_t pieces = 0;
+    for (size_t i = 0; i < items.size(); ++i) {
+        base[i] = (uint32_t)pieces;
+        pieces += std::max<uint64_t>(1, (items[i].len + CRC_PIECE - 1) / CRC_PIECE);
+    }
+    base[items.size()] = (uint32_t)pieces;
+    return pieces < (1ull << 31);
+}
 int crc_upload(pngb200_ctx* ctx, const std::vector<CrcRegion>& regions, uint32_t* d_acc_out, CrcPlan* plan)
 {
     const size_t count = regions.size();
@@ -233,29 +239,22 @@ int crc_upload(pngb200_ctx* ctx, const std::vector<CrcRegion>& regions, uint32_t
     if (count == 0) return PNGB200_OK;
     int rc = ensure_crc_tables(ctx);
     if (rc != PNGB200_OK) return rc;
-    std::vector<uint32_t> base(count + 1);
-    uint64_t pieces = 0;
-    for (size_t i = 0; i < count; ++i) {
-        base[i] = (uint32_t)pieces;
-        pieces += std::max<uint64_t>(1, (regions[i].len + CRC_PIECE - 1) / CRC_PIECE);
-    }
-    base[count] = (uint32_t)pieces;
-    if (pieces >= (1ull << 31)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
-    const size_t rb = sizeof(CrcRegion) * count, off_base = align_up(rb, 256), bb = sizeof(uint32_t) * (count + 1),
-                 off_acc = align_up(off_base + bb, 256), ab = sizeof(uint32_t) * count;
-    CU(ctx->h_crc.reserve(off_acc + ab));
-    CU(ctx->d_crc.reserve(off_acc + ab));
-    memcpy(ctx->h_crc.p, regions.data(), rb);
-    memcpy((char*)ctx->h_crc.p + off_base, base.data(), bb);
-    CU(cudaMemcpyAsync(ctx->d_crc.p, ctx->h_crc.p, off_base + bb, cudaMemcpyHostToDevice, ctx->stream));
-    uint32_t* acc = d_acc_out ? d_acc_out : (uint32_t*)((char*)ctx->d_crc.p + off_acc);
+    std::vector<uint32_t> base;
+    if (!piece_bases(regions, base)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
+    const size_t ab = sizeof(uint32_t) * count;
+    Tables t(ctx->h_crc, ctx->d_crc);
+    const size_t off_regions = t.host(regions.data(), sizeof(CrcRegion) * count);
+    const size_t off_base = t.host(base.data(), sizeof(uint32_t) * (count + 1));
+    const size_t off_acc = t.device(ab, false);
+    if ((rc = t.upload(ctx, t.end)) != PNGB200_OK) return rc;   // crc_fetch brings the results back behind the tables
+    uint32_t* acc = d_acc_out ? d_acc_out : t.dev<uint32_t>(off_acc);
     CU(cudaMemsetAsync(acc, 0, ab, ctx->stream));
-    plan->p.regions = ctx->d_crc.as<CrcRegion>();
-    plan->p.piece_base = (const uint32_t*)((char*)ctx->d_crc.p + off_base);
+    plan->p.regions = t.dev<CrcRegion>(off_regions);
+    plan->p.piece_base = t.dev<uint32_t>(off_base);
     plan->p.acc = acc;
     plan->p.tables = ctx->d_crctab.as<uint32_t>();
     plan->p.count = (uint32_t)count;
-    plan->p.total_pieces = (uint32_t)pieces;
+    plan->p.total_pieces = base[count];
     plan->acc_bytes = ab, plan->off_acc = off_acc;
     return PNGB200_OK;
 }
@@ -300,24 +299,16 @@ int copy_upload(pngb200_ctx* ctx, const std::vector<CopySegment>& segs, CopyPlan
     const size_t count = segs.size();
     plan->any = count != 0;
     if (count == 0) return PNGB200_OK;
-    std::vector<uint32_t> base(count + 1);
-    uint64_t pieces = 0;
-    for (size_t i = 0; i < count; ++i) {
-        base[i] = (uint32_t)pieces;
-        pieces += std::max<uint64_t>(1, (segs[i].len + CRC_PIECE - 1) / CRC_PIECE);
-    }
-    base[count] = (uint32_t)pieces;
-    if (pieces >= (1ull << 31)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
-    const size_t sb = sizeof(CopySegment) * count, off_base = align_up(sb, 256), bb = sizeof(uint32_t) * (count + 1);
-    CU(ctx->h_seg.reserve(off_base + bb));
-    CU(ctx->d_seg.reserve(off_base + bb));
-    memcpy(ctx->h_seg.p, segs.data(), sb);
-    memcpy((char*)ctx->h_seg.p + off_base, base.data(), bb);
-    CU(cudaMemcpyAsync(ctx->d_seg.p, ctx->h_seg.p, off_base + bb, cudaMemcpyHostToDevice, ctx->stream));
-    plan->p.segments = ctx->d_seg.as<CopySegment>();
-    plan->p.piece_base = (const uint32_t*)((char*)ctx->d_seg.p + off_base);
+    std::vector<uint32_t> base;
+    if (!piece_bases(segs, base)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
+    Tables t(ctx->h_seg, ctx->d_seg);
+    const size_t off_segs = t.host(segs.data(), sizeof(CopySegment) * count);
+    const size_t off_base = t.host(base.data(), sizeof(uint32_t) * (count + 1));
+    if (int rc = t.upload(ctx)) return rc;
+    plan->p.segments = t.dev<CopySegment>(off_segs);
+    plan->p.piece_base = t.dev<uint32_t>(off_base);
     plan->p.count = (uint32_t)count;
-    plan->p.total_pieces = (uint32_t)pieces;
+    plan->p.total_pieces = base[count];
     return PNGB200_OK;
 }
 int copy_launch(pngb200_ctx* ctx, const CopyPlan& plan)
@@ -350,7 +341,7 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
     // does the concatenation: a run of equal-sized IDAT chunks (what every encoder writes, the reference
     // included) is one pitched copy (cudaMemcpy2DAsync: row = body, source pitch = body + 12).
     std::vector<size_t> f_off(count), g_off(count), pre_len(count), post_at(count), post_len(count);
-    size_t f_total = 0, g_total = 0;
+    Slots files{16}, payloads{16};
     for (size_t i = 0; i < count; ++i) {
         if (!d[i].file && d[i].file_len) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "file %zu: null pointer", i);
         FileWalk& w = walks[i];
@@ -369,13 +360,11 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
             post_at[i] = w.idat_end < w.chunks.size() ? (size_t)w.chunks[w.idat_end].off : lexed;
             post_len[i] = lexed - post_at[i];
         }
-        f_off[i] = f_total;
-        f_total += align_up(pre_len[i] + post_len[i] + 16, 256);
-        g_off[i] = g_total;
-        g_total += align_up(d[i].idat_bytes + 16, 256);
+        f_off[i] = files.add(pre_len[i] + post_len[i]);
+        g_off[i] = payloads.add(d[i].idat_bytes);
     }
-    CU(ctx->d_file.reserve(std::max<size_t>(f_total, 256)));
-    CU(ctx->d_in.reserve(std::max<size_t>(g_total, 256)));
+    CU(ctx->d_file.reserve(std::max<size_t>(files.total, 256)));
+    CU(ctx->d_in.reserve(std::max<size_t>(payloads.total, 256)));
     // every lexed chunk's CRC region (type + body): in the file arena, or -- IDAT run -- the body in the
     // payload arena with the type folded in as a prefix
     std::vector<CrcRegion> regions;
@@ -438,7 +427,7 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
     std::vector<pngb200_image_desc> images;
     std::vector<size_t>             owner;
     std::vector<size_t>             o_off(count);
-    size_t o_total = 0;
+    Slots outs{16};
     for (size_t i = 0; i < count; ++i) {
         const FileWalk& w = walks[i];
         Plan& p = plans[i];
@@ -463,21 +452,19 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
         memset(&im, 0, sizeof im);
         im.idat = ctx->d_in.as<uint8_t>() + g_off[i];  // the chunks pushed so far are a prefix of the gathered run
         im.idat_len = payload;
-        if (host_pixels) {
-            o_off[i] = o_total;
-            o_total += align_up(d[i].storage_size + 16, 256);
-        } else {
+        if (host_pixels)
+            o_off[i] = outs.add(d[i].storage_size);
+        else
             im.pixels = (uint8_t*)d[i].pixels;
-        }
         im.pixels_cap = d[i].storage_size;
         im.width = d[i].width, im.height = d[i].height;
-        im.volume = (uint8_t)(d[i].depth * channels_of_color(d[i].color)), im.depth = d[i].depth;
+        im.volume = (uint8_t)(d[i].depth * pixel_rule(d[i].color, d[i].depth, false).channels), im.depth = d[i].depth;
         im.interlaced = d[i].interlaced;
         im.format = d[i].standard ? PNGB200_FORMAT_IOS : PNGB200_FORMAT_ZLIB;
         images.push_back(im);
         owner.push_back(i);
     }
-    if (o_total) CU(ctx->d_out.reserve(o_total));
+    if (outs.total) CU(ctx->d_out.reserve(outs.total));
     if (host_pixels)
         for (size_t j = 0; j < images.size(); ++j) images[j].pixels = ctx->d_out.as<uint8_t>() + o_off[owner[j]];
     CrcPlan crc_plan;
@@ -581,7 +568,7 @@ size_t pngb200_png_encode_bound(uint32_t width, uint32_t height, const pngb200_p
 {
     if (!f) return 0;
     const size_t chunk = idat_chunk ? idat_chunk : 65544;
-    const int    volume = f->depth * channels_of_color(f->color);
+    const int    volume = f->depth * pixel_rule(f->color, f->depth, false).channels;
     const size_t z = pngb200_deflate_bound(pngb200_filtered_size(width, height, volume, interlaced));
     return 8 + 16 + 25 + (12 + 768) + (12 + 256) + z + 12 * (z / chunk + 2) + 12 + 64;
 }
@@ -597,32 +584,26 @@ int pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_
     std::vector<pngb200_encode_desc> enc(count);
     std::vector<size_t> p_off(count), z_off(count), head_len(count);
     std::vector<std::vector<uint8_t>> heads(count);
-    size_t p_total = 0, z_total = 0;
+    Slots pixels{16}, payloads{16};
     for (size_t i = 0; i < count; ++i) {
         const pngb200_pixel_format& f = d[i].format;
-        const int ch = f.color == 0 || f.color == 3 ? 1 : f.color == 2 ? 3 : f.color == 4 ? 2 : f.color == 6 ? 4 : 0;
-        const bool depth_ok = f.color == 3 ? (f.depth == 1 || f.depth == 2 || f.depth == 4 || f.depth == 8)
-                            : f.color == 0 ? (f.depth == 1 || f.depth == 2 || f.depth == 4 || f.depth == 8 || f.depth == 16)
-                                           : (f.depth == 8 || f.depth == 16);
-        if (!ch || !depth_ok || !d[i].width || !d[i].height || !d[i].pixels || !d[i].file ||
-            (f.bgr && (f.depth != 8 || (f.color != 2 && f.color != 6))) ||
+        const PixelRule rule = pixel_rule(f.color, f.depth, f.bgr);
+        if (!rule.valid || !d[i].width || !d[i].height || !d[i].pixels || !d[i].file ||
             (f.color == 3 && (!f.palette || !f.palette_count || f.palette_count > (1u << f.depth))))
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: bad descriptor", i);
-        const int    volume = f.depth * ch;
+        const int    volume = f.depth * rule.channels;
         const size_t storage = pngb200_storage_size(d[i].width, d[i].height, volume);
         if (d[i].pixels_len < storage) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: pixels_len", i);
         if (d[i].file_cap < pngb200_png_encode_bound(d[i].width, d[i].height, &f, d[i].interlaced, d[i].idat_chunk))
             return set_error(ctx, PNGB200_ERR_OUTPUT_CAPACITY, "image %zu: file_cap below pngb200_png_encode_bound", i);
-        p_off[i] = p_total;
-        p_total += align_up(storage + 16, 256);
-        z_off[i] = z_total;
-        z_total += align_up(pngb200_deflate_bound(pngb200_filtered_size(d[i].width, d[i].height, volume, d[i].interlaced)) + 16, 256);
+        p_off[i] = pixels.add(storage);
+        z_off[i] = payloads.add(pngb200_deflate_bound(pngb200_filtered_size(d[i].width, d[i].height, volume, d[i].interlaced)));
     }
-    if (host_pixels) CU(ctx->d_in.reserve(p_total));
-    CU(ctx->d_out.reserve(z_total));
+    if (host_pixels) CU(ctx->d_in.reserve(pixels.total));
+    CU(ctx->d_out.reserve(payloads.total));
     for (size_t i = 0; i < count; ++i) {
         const pngb200_pixel_format& f = d[i].format;
-        const int    volume = f.depth * channels_of_color(f.color);
+        const int    volume = f.depth * pixel_rule(f.color, f.depth, f.bgr).channels;
         const size_t storage = pngb200_storage_size(d[i].width, d[i].height, volume);
         pngb200_encode_desc& e = enc[i];
         memset(&e, 0, sizeof e);
@@ -691,20 +672,19 @@ int pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_
     if (rc != PNGB200_OK) return rc;
     // stage 2: frame the payload into IDAT chunks inside a device image of the file, CRC them there
     std::vector<size_t> file_off(count), file_len(count);
-    size_t file_total = 0;
+    Slots files{16};
     std::vector<FrameItem>   frames;
     std::vector<CrcRegion>   regions;
     std::vector<CopySegment> segs;
     for (size_t i = 0; i < count; ++i) {
         d[i].status = enc[i].status, d[i].checksum = enc[i].checksum, d[i].blocks = enc[i].blocks, d[i].produced = 0;
-        file_off[i] = file_total;
-        if (enc[i].status != PNGB200_OK) { file_len[i] = 0; continue; }
+        if (enc[i].status != PNGB200_OK) continue;
         const size_t chunk = d[i].idat_chunk ? d[i].idat_chunk : 65544;
         const size_t z = enc[i].produced, nchunks = (z + chunk - 1) / chunk;
         file_len[i] = head_len[i] + z + 12 * nchunks + 12;
-        file_total += align_up(file_len[i] + 16, 256);
+        file_off[i] = files.add(file_len[i]);
     }
-    CU(ctx->d_file.reserve(std::max<size_t>(file_total, 256)));
+    CU(ctx->d_file.reserve(std::max<size_t>(files.total, 256)));
     for (size_t i = 0; i < count; ++i) {
         if (enc[i].status != PNGB200_OK) continue;
         uint8_t* base = ctx->d_file.as<uint8_t>() + file_off[i];
@@ -727,18 +707,18 @@ int pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_
     rc = run_segment_copy(ctx, segs);
     if (rc != PNGB200_OK) return rc;
     if (!frames.empty()) {
-        const size_t fb = sizeof(FrameItem) * frames.size(), off_crc = align_up(fb, 256), cb = sizeof(uint32_t) * frames.size();
-        CU(ctx->h_genjobs.reserve(fb));
-        CU(ctx->d_genjobs.reserve(off_crc + cb));
-        memcpy(ctx->h_genjobs.p, frames.data(), fb);
-        CU(cudaMemcpyAsync(ctx->d_genjobs.p, ctx->h_genjobs.p, fb, cudaMemcpyHostToDevice, ctx->stream));
-        uint32_t* d_crc = (uint32_t*)((char*)ctx->d_genjobs.p + off_crc);
+        Tables t(ctx->h_genjobs, ctx->d_genjobs);
+        const size_t off_frames = t.host(frames.data(), sizeof(FrameItem) * frames.size());
+        const size_t off_crc = t.device(sizeof(uint32_t) * frames.size(), false);   // run_crc clears it
+        if ((rc = t.upload(ctx)) != PNGB200_OK) return rc;
+        FrameItem* d_frames = t.dev<FrameItem>(off_frames);
+        uint32_t*  d_crc = t.dev<uint32_t>(off_crc);
         const unsigned blocks = (unsigned)((frames.size() + 255) / 256);
-        frame_chunks_kernel<<<blocks, 256, 0, ctx->stream>>>(ctx->d_genjobs.as<FrameItem>(), d_crc, (uint32_t)frames.size(), 0);
+        frame_chunks_kernel<<<blocks, 256, 0, ctx->stream>>>(d_frames, d_crc, (uint32_t)frames.size(), 0);
         ctx->launches++;
         rc = run_crc(ctx, regions, d_crc, nullptr);  // the chunk type is folded in as a 4-byte prefix
         if (rc != PNGB200_OK) return rc;
-        frame_chunks_kernel<<<blocks, 256, 0, ctx->stream>>>(ctx->d_genjobs.as<FrameItem>(), d_crc, (uint32_t)frames.size(), 1);
+        frame_chunks_kernel<<<blocks, 256, 0, ctx->stream>>>(d_frames, d_crc, (uint32_t)frames.size(), 1);
         ctx->launches++;
         CU(cudaGetLastError());
     }

@@ -34,57 +34,64 @@ namespace {
 
 thread_local std::string g_last_error;
 
-struct DevBuf {
+// A grow-only workspace that owns its memory: device memory (cudaMalloc) or pinned host memory (cudaHostAlloc).
+// Movable, not copyable; a move assignment swaps, so the buffer moved from frees the old memory when it goes.
+template <bool Pinned>
+struct Buf {
     void*  p   = nullptr;
     size_t cap = 0;
+    Buf() = default;
+    Buf(Buf&& o) noexcept { std::swap(p, o.p), std::swap(cap, o.cap); }
+    Buf& operator=(Buf&& o) noexcept
+    {
+        std::swap(p, o.p), std::swap(cap, o.cap);
+        return *this;
+    }
+    ~Buf() { release(); }
     cudaError_t reserve(size_t n)
     {
         if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        size_t want = std::max(n + std::min(n / 4, (size_t)1 << 30), (size_t)1 << 16);
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e != cudaSuccess) {
-            want = n;
+        release();
+        size_t      want;
+        cudaError_t e;
+        if (Pinned) {
+            want = std::max(n + n / 4, (size_t)1 << 12);
+            e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
+        } else {
+            want = std::max(n + std::min(n / 4, (size_t)1 << 30), (size_t)1 << 16);
             e = cudaMalloc(&p, want);
+            if (e != cudaSuccess) {
+                want = n;
+                e = cudaMalloc(&p, want);
+            }
         }
         if (e == cudaSuccess) cap = want;
         return e;
     }
     void release()
     {
-        if (p) cudaFree(p);
+        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
         p = nullptr;
         cap = 0;
     }
     template <typename T> T* as() const { return (T*)p; }
 };
-
-struct PinBuf {
-    void*  p   = nullptr;
-    size_t cap = 0;
-    cudaError_t reserve(size_t n)
-    {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-        size_t want = std::max(n + n / 4, (size_t)1 << 12);
-        cudaError_t e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    void release()
-    {
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-    }
-    template <typename T> T* as() const { return (T*)p; }
-};
+using DevBuf = Buf<false>;
+using PinBuf = Buf<true>;
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Per-item staging slots of an arena: the item's bytes plus `pad`, rounded up to 256
+struct Slots {
+    size_t pad;
+    size_t total = 0;
+    size_t add(size_t bytes)   // the item's offset
+    {
+        const size_t off = total;
+        total += align_up(bytes + pad, 256);
+        return off;
+    }
+};
 
 const int ADAM7[7][4] = {{0, 0, 3, 3}, {4, 0, 3, 3}, {0, 4, 2, 3}, {2, 0, 2, 2},
                          {0, 2, 1, 2}, {1, 0, 1, 1}, {0, 1, 0, 1}};
@@ -165,6 +172,64 @@ struct DeviceGuard {
         if (prev >= 0) cudaSetDevice(prev);
     }
 };
+
+// The small tables of a launch, uploaded with one H2D copy: host arrays, then device-only regions, each at a
+// 256-byte-aligned offset of a device buffer.  upload() packs the host arrays into the pinned buffer, copies that
+// part, and clears the device-only regions asked to be zero; it may move both buffers, so dev() and pin() are for
+// after it.  A pinned buffer must not take a second table before a stream synchronise: the copy reads it when the
+// stream gets there.
+struct Tables {
+    PinBuf& h;
+    DevBuf& d;
+    struct Part { const void* src; size_t off, bytes; bool zero; };
+    std::vector<Part> parts;
+    size_t host_end = 0, end = 0;
+    Tables(PinBuf& h_, DevBuf& d_) : h(h_), d(d_) {}
+    size_t host(const void* src, size_t bytes)   // src null: the region is copied unwritten
+    {
+        const size_t off = add(src, bytes, false);
+        host_end = end;
+        return off;
+    }
+    size_t device(size_t bytes, bool zero) { return add(nullptr, bytes, zero); }
+    size_t add(const void* src, size_t bytes, bool zero)
+    {
+        const size_t off = align_up(end, 256);
+        parts.push_back({src, off, bytes, zero});
+        end = off + bytes;
+        return off;
+    }
+    // `pinned`: bytes of pinned memory to reserve when a readback lands behind the host arrays
+    int upload(pngb200_ctx* ctx, size_t pinned = 0)
+    {
+        CU(h.reserve(std::max(pinned, host_end)));
+        CU(d.reserve(end));
+        for (const Part& p : parts)
+            if (p.src && p.bytes) memcpy((char*)h.p + p.off, p.src, p.bytes);
+        CU(cudaMemcpyAsync(d.p, h.p, host_end, cudaMemcpyHostToDevice, ctx->stream));
+        for (const Part& p : parts)
+            if (p.zero) CU(cudaMemsetAsync((char*)d.p + p.off, 0, p.bytes, ctx->stream));
+        return PNGB200_OK;
+    }
+    template <typename T> T* dev(size_t off) const { return (T*)((char*)d.p + off); }
+    template <typename T> T* pin(size_t off) const { return (T*)((char*)h.p + off); }
+};
+
+// PNG.Format.Pixel.recognize(code:): whether (color, depth, bgr) is a pixel format (bgr, the iOS byte order: 8-bit
+// RGB and RGBA only), and the channels of colour type `color` (4 for a type that does not exist)
+struct PixelRule { bool valid; int channels; };
+PixelRule pixel_rule(int color, int depth, bool bgr)
+{
+    bool ok;
+    switch (color) {
+    case 0: ok = depth == 1 || depth == 2 || depth == 4 || depth == 8 || depth == 16; break;
+    case 3: ok = depth == 1 || depth == 2 || depth == 4 || depth == 8; break;
+    case 2: case 4: case 6: ok = depth == 8 || depth == 16; break;
+    default: ok = false;
+    }
+    if (bgr && (depth != 8 || (color != 2 && color != 6))) ok = false;
+    return {ok, color == 0 || color == 3 ? 1 : color == 2 ? 3 : color == 4 ? 2 : 4};
+}
 
 // the CRC-32 byte table and shift operators (crc32.cuh), uploaded once per context
 int ensure_crc_tables(pngb200_ctx* ctx)
@@ -379,22 +444,18 @@ int run_segments(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t
     if (!recs.empty()) {
         // 4. windows in front of the segments, then markers -> bytes at their final places
         const size_t nr = recs.size(), ns = stream_first.size() - 1;
-        const size_t off_first = align_up(sizeof(SegmentRecord) * nr, 256);
-        const size_t off_chunk = align_up(off_first + sizeof(uint32_t) * (ns + 1), 256);
-        const size_t table = off_chunk + sizeof(uint64_t) * nr;
-        CU(ctx->h_sgrec.reserve(table));
-        CU(ctx->d_sgrec.reserve(table));
-        memcpy(ctx->h_sgrec.p, recs.data(), sizeof(SegmentRecord) * nr);
-        memcpy((char*)ctx->h_sgrec.p + off_first, stream_first.data(), sizeof(uint32_t) * (ns + 1));
-        memcpy((char*)ctx->h_sgrec.p + off_chunk, chunk_base.data(), sizeof(uint64_t) * nr);
-        CU(cudaMemcpyAsync(ctx->d_sgrec.p, ctx->h_sgrec.p, table, cudaMemcpyHostToDevice, ctx->stream));
+        Tables t(ctx->h_sgrec, ctx->d_sgrec);
+        const size_t off_recs = t.host(recs.data(), sizeof(SegmentRecord) * nr);
+        const size_t off_first = t.host(stream_first.data(), sizeof(uint32_t) * (ns + 1));
+        const size_t off_chunk = t.host(chunk_base.data(), sizeof(uint64_t) * nr);
+        if (int rc = t.upload(ctx)) return rc;
         CU(ctx->d_sgwin.reserve((size_t)SEG_WINDOW * nr));
-        const SegmentRecord* d_recs = ctx->d_sgrec.as<SegmentRecord>();
-        window_propagate_kernel<<<(unsigned)ns, 256, 0, ctx->stream>>>(d_recs, (const uint32_t*)((char*)ctx->d_sgrec.p + off_first),
-                                                                       (uint32_t)ns, ctx->d_sgwin.as<uint8_t>());
+        const SegmentRecord* d_recs = t.dev<SegmentRecord>(off_recs);
+        window_propagate_kernel<<<(unsigned)ns, 256, 0, ctx->stream>>>(d_recs, t.dev<uint32_t>(off_first), (uint32_t)ns,
+                                                                       ctx->d_sgwin.as<uint8_t>());
         if (chunks)
             marker_resolve_kernel<<<(unsigned)chunks, 256, 0, ctx->stream>>>(d_recs, (uint32_t)nr, ctx->d_sgwin.as<uint8_t>(),
-                                                                             (const uint64_t*)((char*)ctx->d_sgrec.p + off_chunk));
+                                                                             t.dev<uint64_t>(off_chunk));
         ctx->launches += 2;
         CU(cudaGetLastError());
         // the streams' result records (the whole-stream kernels will not touch them)
@@ -499,27 +560,26 @@ int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& 
                               (unsigned)std::min<size_t>(2 * n, slots), max_cap, d_switch))
         return rc;
     // 3. tails -> bytes behind their heads, Adler-32 of the whole stream, acceptance; device-side, one host round trip
-    const size_t off_accept  = align_up(sizeof(SplitRecord) * n, 256);
-    const size_t off_partial = align_up(off_accept + sizeof(uint32_t) * n, 256);
-    const size_t table       = off_partial + sizeof(uint32_t) * 2 * SPLIT_CTAS * n;
-    CU(ctx->h_sgrec.reserve(off_partial));
-    CU(ctx->d_sgrec.reserve(table));
-    SplitRecord* rec = ctx->h_sgrec.as<SplitRecord>();
+    std::vector<SplitRecord> rec(n);
     const StreamResult* d_sgres = ctx->d_sgres.as<StreamResult>();
     for (size_t s = 0; s < n; ++s) {
         const StreamJob& j = h_jobs[cut[s]];
         rec[s] = SplitRecord{d_sgres + s, d_sgres + n + s, (const uint16_t*)j.scratch, j.dst, j.dst_cap, sg[s].stop_bit,
                              ctx->d_results.as<StreamResult>() + cut[s], d_switch + n + s};
     }
-    CU(cudaMemcpyAsync(ctx->d_sgrec.p, rec, sizeof(SplitRecord) * n, cudaMemcpyHostToDevice, ctx->stream));
-    const SplitRecord* d_rec = ctx->d_sgrec.as<SplitRecord>();
-    uint32_t* d_accept  = (uint32_t*)((char*)ctx->d_sgrec.p + off_accept);
-    uint32_t* d_partial = (uint32_t*)((char*)ctx->d_sgrec.p + off_partial);
+    Tables t(ctx->h_sgrec, ctx->d_sgrec);
+    const size_t off_rec = t.host(rec.data(), sizeof(SplitRecord) * n);
+    const size_t off_accept = t.device(sizeof(uint32_t) * n, false);
+    const size_t off_partial = t.device(sizeof(uint32_t) * 2 * SPLIT_CTAS * n, false);
+    if (int rc = t.upload(ctx, off_partial)) return rc;   // the accept flags come back behind the records
+    const SplitRecord* d_rec = t.dev<SplitRecord>(off_rec);
+    uint32_t* d_accept  = t.dev<uint32_t>(off_accept);
+    uint32_t* d_partial = t.dev<uint32_t>(off_partial);
     split_resolve_kernel<<<dim3((unsigned)n, SPLIT_CTAS), 256, 0, ctx->stream>>>(d_rec, d_partial);
     split_finish_kernel<<<(unsigned)((n + 127) / 128), 128, 0, ctx->stream>>>(d_rec, (uint32_t)n, d_partial, d_accept);
     ctx->launches += 2;
     CU(cudaGetLastError());
-    uint32_t* accept = (uint32_t*)((char*)ctx->h_sgrec.p + off_accept);
+    uint32_t* accept = t.pin<uint32_t>(off_accept);
     CU(cudaMemcpyAsync(accept, d_accept, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
     CU(ctx->h_sgres.reserve(res_bytes));
     CU(cudaMemcpyAsync(ctx->h_sgres.p, d_sgres, res_bytes, cudaMemcpyDeviceToHost, ctx->stream));
@@ -550,6 +610,45 @@ int run_split(pngb200_ctx* ctx, const StreamJob* h_jobs, std::vector<uint32_t>& 
     for (uint32_t i : par)
         if (std::find(rest.begin(), rest.end(), i) != rest.end()) left.push_back(i);
     par.swap(left);
+    return PNGB200_OK;
+}
+
+// Stream checksums (Adler-32, CRC-32 for gzip) of `count` inflated jobs, in chunks laid out from dst_cap (an upper
+// bound of `produced`).  `h_base`: count + 1 words of host staging for the chunk bases, uploaded to `d_base`.
+int run_checksum(pngb200_ctx* ctx, const StreamJob* h_jobs, const StreamJob* d_jobs, StreamResult* d_results, size_t count,
+                 uint32_t* h_base, DevBuf& d_base, DevBuf& d_partial)
+{
+    uint64_t total = 0;
+    for (size_t i = 0; i < count; ++i) {
+        h_base[i] = (uint32_t)total;
+        total += (h_jobs[i].dst_cap + CK_CHUNK - 1) / CK_CHUNK;
+    }
+    h_base[count] = (uint32_t)total;
+    if (total >= (1ull << 31)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
+    CU(d_base.reserve(sizeof(uint32_t) * (count + 1)));
+    CU(d_partial.reserve(sizeof(uint64_t) * 2 * std::max<uint64_t>(total, 1)));
+    CU(cudaMemcpyAsync(d_base.p, h_base, sizeof(uint32_t) * (count + 1), cudaMemcpyHostToDevice, ctx->stream));
+    ChecksumParams cp;
+    cp.jobs = d_jobs;
+    cp.results = d_results;
+    cp.chunk_base = d_base.as<uint32_t>();
+    cp.partial = d_partial.as<uint64_t>();
+    cp.count = (uint32_t)count;
+    cp.total_chunks = (uint32_t)total;
+    cp.crc_tables = nullptr;
+    for (size_t i = 0; i < count; ++i)
+        if (h_jobs[i].format == PNGB200_FORMAT_GZIP) {
+            if (int rc = ensure_crc_tables(ctx)) return rc;
+            cp.crc_tables = ctx->d_crctab.as<uint32_t>();
+            break;
+        }
+    if (total) {
+        checksum_chunk_kernel<<<(unsigned)total, CK_THREADS, 0, ctx->stream>>>(cp);
+        ctx->launches++;
+    }
+    checksum_fold_kernel<<<(unsigned)count, 32, 0, ctx->stream>>>(cp);
+    ctx->launches++;
+    CU(cudaGetLastError());
     return PNGB200_OK;
 }
 
@@ -647,41 +746,9 @@ int run_inflate(pngb200_ctx* ctx, const StreamJob* h_jobs, size_t count)
         CU(cudaGetLastError());
     }
     CU(cudaEventRecord(ctx->ev[1], ctx->stream));
-    // checksum: chunk layout from dst_cap (an upper bound of `produced`)
     CU(ctx->h_misc.reserve(sizeof(uint32_t) * (count + 1)));
-    uint32_t* base = ctx->h_misc.as<uint32_t>();
-    uint64_t  total = 0;
-    for (size_t i = 0; i < count; ++i) {
-        base[i] = (uint32_t)total;
-        total += (h_jobs[i].dst_cap + CK_CHUNK - 1) / CK_CHUNK;
-    }
-    base[count] = (uint32_t)total;
-    if (total >= (1ull << 31)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
-    CU(ctx->d_misc.reserve(sizeof(uint32_t) * (count + 1)));
-    CU(ctx->d_partial.reserve(sizeof(uint64_t) * 2 * std::max<uint64_t>(total, 1)));
-    CU(cudaMemcpyAsync(ctx->d_misc.p, base, sizeof(uint32_t) * (count + 1), cudaMemcpyHostToDevice,
-                       ctx->stream));
-    ChecksumParams cp;
-    cp.jobs = d_jobs;
-    cp.results = d_results;
-    cp.chunk_base = ctx->d_misc.as<uint32_t>();
-    cp.partial = ctx->d_partial.as<uint64_t>();
-    cp.count = (uint32_t)count;
-    cp.total_chunks = (uint32_t)total;
-    cp.crc_tables = nullptr;
-    for (size_t i = 0; i < count; ++i)
-        if (h_jobs[i].format == PNGB200_FORMAT_GZIP) {
-            if (int rc = ensure_crc_tables(ctx)) return rc;
-            cp.crc_tables = ctx->d_crctab.as<uint32_t>();
-            break;
-        }
-    if (total) {
-        checksum_chunk_kernel<<<(unsigned)total, CK_THREADS, 0, ctx->stream>>>(cp);
-        ctx->launches++;
-    }
-    checksum_fold_kernel<<<(unsigned)count, 32, 0, ctx->stream>>>(cp);
-    ctx->launches++;
-    CU(cudaGetLastError());
+    if (int rc = run_checksum(ctx, h_jobs, d_jobs, d_results, count, ctx->h_misc.as<uint32_t>(), ctx->d_misc, ctx->d_partial))
+        return rc;
     CU(cudaEventRecord(ctx->ev[2], ctx->stream));
     return PNGB200_OK;
 }
@@ -797,28 +864,25 @@ int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
                 }
             }
         }
-        size_t jb = sizeof(ImageJob) * fast.size(), bb = sizeof(uint32_t) * band_base.size();
-        size_t lb = sizeof(uint32_t) * level_start.size();
-        size_t off_bb = align_up(jb, 256), off_ls = align_up(off_bb + bb, 256), off_pr = align_up(off_ls + lb, 256);
-        size_t total = align_up(off_pr + sizeof(uint32_t) * (bands + 1), 8) + 8 * sizeof(unsigned long long);
-        CU(ctx->h_imgjobs.reserve(off_pr));
-        CU(ctx->d_imgjobs.reserve(total));
-        memcpy(ctx->h_imgjobs.p, fast.data(), jb);
-        memcpy((char*)ctx->h_imgjobs.p + off_bb, band_base.data(), bb);
-        if (lb) memcpy((char*)ctx->h_imgjobs.p + off_ls, level_start.data(), lb);
-        CU(cudaMemcpyAsync(ctx->d_imgjobs.p, ctx->h_imgjobs.p, off_pr, cudaMemcpyHostToDevice, ctx->stream));
-        CU(cudaMemsetAsync((char*)ctx->d_imgjobs.p + off_pr, 0, sizeof(uint32_t) * (bands + 1), ctx->stream));
+        Tables t(ctx->h_imgjobs, ctx->d_imgjobs);
+        const size_t off_jobs = t.host(fast.data(), sizeof(ImageJob) * fast.size());
+        const size_t off_bb = t.host(band_base.data(), sizeof(uint32_t) * band_base.size());
+        const size_t off_ls = t.host(level_start.data(), sizeof(uint32_t) * level_start.size());
+        t.host(nullptr, 0);   // the copy runs on up to the counters
+        // per-band progress and the ticket, padded to 8 bytes, then the filter-type histogram: one zeroed region
+        const size_t progress = sizeof(uint32_t) * ((bands + 2) / 2 * 2);
+        const size_t off_pr = t.device(progress + 8 * sizeof(unsigned long long), true);
+        if (int rc = t.upload(ctx)) return rc;
         WaveParams p;
-        p.jobs = ctx->d_imgjobs.as<ImageJob>();
-        p.band_base = (const uint32_t*)((char*)ctx->d_imgjobs.p + off_bb);
-        p.progress = (uint32_t*)((char*)ctx->d_imgjobs.p + off_pr);
+        p.jobs = t.dev<ImageJob>(off_jobs);
+        p.band_base = t.dev<uint32_t>(off_bb);
+        p.progress = t.dev<uint32_t>(off_pr);
         p.ticket = p.progress + bands;
-        p.hist = (unsigned long long*)((char*)ctx->d_imgjobs.p + align_up(off_pr + sizeof(uint32_t) * (bands + 1), 8));
-        CU(cudaMemsetAsync(p.hist, 0, 8 * sizeof(unsigned long long), ctx->stream));
+        p.hist = t.dev<unsigned long long>(off_pr + progress);
         ctx->d_hist = p.hist;
         p.njobs = (uint32_t)fast.size();
         p.total_bands = (uint32_t)bands;
-        p.level_start = (const uint32_t*)((char*)ctx->d_imgjobs.p + off_ls);
+        p.level_start = t.dev<uint32_t>(off_ls);
         p.levels = level_start.empty() ? 0u : (uint32_t)level_start.size() - 1;
         unsigned grid = (unsigned)std::min<uint64_t>((bands + WAVE_WARPS - 1) / WAVE_WARPS,
                                                      (uint64_t)ctx->sm_count * 8);
@@ -827,13 +891,10 @@ int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
         CU(cudaGetLastError());
     }
     if (!slow.empty()) {
-        size_t jb = sizeof(GenericJob) * slow.size();
-        CU(ctx->h_genjobs.reserve(jb));
-        CU(ctx->d_genjobs.reserve(jb));
-        memcpy(ctx->h_genjobs.p, slow.data(), jb);
-        CU(cudaMemcpyAsync(ctx->d_genjobs.p, ctx->h_genjobs.p, jb, cudaMemcpyHostToDevice, ctx->stream));
-        unfilter_generic_kernel<<<(unsigned)slow.size(), 128, 0, ctx->stream>>>(
-            ctx->d_genjobs.as<GenericJob>(), (int)slow.size());
+        Tables t(ctx->h_genjobs, ctx->d_genjobs);
+        const size_t off_jobs = t.host(slow.data(), sizeof(GenericJob) * slow.size());
+        if (int rc = t.upload(ctx)) return rc;
+        unfilter_generic_kernel<<<(unsigned)slow.size(), 128, 0, ctx->stream>>>(t.dev<GenericJob>(off_jobs), (int)slow.size());
         ctx->launches++;
         CU(cudaGetLastError());
     }
@@ -957,31 +1018,17 @@ pngb200_ctx* pngb200_ctx_create(int device)
     if (const char* v = getenv("PNGB200_SPLIT")) ctx->split = atoi(v) != 0;   // tuning overrides, read once per context
     if (const char* v = getenv("PNGB200_PLAN_SLOTS")) ctx->plan_slots = (size_t)std::max(0, atoi(v));
     DeviceGuard guard(device);
-    if (cudaFuncSetAttribute(deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DfShared)) != cudaSuccess) {
-        set_error(nullptr, PNGB200_ERR_CUDA, "cannot opt in to %zu bytes of shared memory", sizeof(DfShared));
-        delete ctx;
-        return nullptr;
-    }
-    if (configure_inflate_parallel() != 0) {
-        set_error(nullptr, PNGB200_ERR_CUDA, "cannot opt in to %zu bytes of shared memory", sizeof(ParShared));
-        delete ctx;
-        return nullptr;
-    }
-    if (configure_inflate_wave() != 0) {
-        set_error(nullptr, PNGB200_ERR_CUDA, "cannot opt in to %zu bytes of shared memory", sizeof(WvShared));
-        delete ctx;
-        return nullptr;
-    }
-    if (cudaFuncSetAttribute(unfilter_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WAVE_SMEM) != cudaSuccess) {
-        set_error(nullptr, PNGB200_ERR_CUDA, "cannot opt in to %zu bytes of shared memory", (size_t)WAVE_SMEM);
-        delete ctx;
-        return nullptr;
-    }
-    if (configure_inflate_cells() != 0) {
-        set_error(nullptr, PNGB200_ERR_CUDA, "cannot opt in to %zu bytes of shared memory", sizeof(ClShared));
-        delete ctx;
-        return nullptr;
-    }
+    // each kernel launched with dynamic shared memory opts in to its size
+    const std::pair<const void*, size_t> opt_in[] = {
+        {(const void*)deflate_kernel, sizeof(DfShared)},          {(const void*)inflate_parallel_kernel3, sizeof(ParShared)},
+        {(const void*)inflate_parallel_kernel, sizeof(ParShared)}, {(const void*)inflate_wave_kernel, sizeof(WvShared)},
+        {(const void*)unfilter_wave_kernel, WAVE_SMEM},           {(const void*)inflate_cells_kernel, sizeof(ClShared)}};
+    for (const auto& [kernel, bytes] : opt_in)
+        if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess) {
+            set_error(nullptr, PNGB200_ERR_CUDA, "cannot opt in to %zu bytes of shared memory", bytes);
+            delete ctx;
+            return nullptr;
+        }
     if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {
         set_error(nullptr, PNGB200_ERR_CUDA, "cudaStreamCreate failed");
         delete ctx;
@@ -998,17 +1045,9 @@ void pngb200_ctx_destroy(pngb200_ctx* ctx)
     ctx->lanes.clear();
     DeviceGuard guard(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    for (DevBuf* b : {&ctx->d_jobs, &ctx->d_results, &ctx->d_imgjobs, &ctx->d_genjobs, &ctx->d_misc,
-                      &ctx->d_partial, &ctx->d_filtered, &ctx->d_in, &ctx->d_out, &ctx->d_order, &ctx->d_scratch, &ctx->d_dfscratch,
-                      &ctx->d_dfjobs, &ctx->d_dfres, &ctx->d_enc, &ctx->d_file, &ctx->d_crc, &ctx->d_seg, &ctx->d_crctab,
-                      &ctx->d_sgjobs, &ctx->d_sgres, &ctx->d_sgsym, &ctx->d_sgsearch, &ctx->d_sgrec, &ctx->d_sgwin})
-        b->release();
-    for (PinBuf* b : {&ctx->h_jobs, &ctx->h_results, &ctx->h_imgjobs, &ctx->h_genjobs, &ctx->h_misc, &ctx->h_order, &ctx->h_crc, &ctx->h_seg,
-                      &ctx->h_sgsearch, &ctx->h_sgjobs, &ctx->h_sgres, &ctx->h_sgrec})
-        b->release();
     for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
     cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;   // frees the workspaces
 }
 
 int pngb200_ctx_trim(pngb200_ctx* ctx)
@@ -1129,18 +1168,16 @@ int pngb200_inflate_batch(pngb200_ctx* ctx, pngb200_stream_desc* s, size_t count
     CU(ctx->h_results.reserve(sizeof(StreamResult) * count));
     StreamJob* jobs = ctx->h_jobs.as<StreamJob>();
     std::vector<size_t> in_off(count), out_off(count);
-    size_t in_total = 0, out_total = 0;
+    Slots in{16}, out{16};
     for (size_t i = 0; i < count; ++i) {
         if ((!s[i].src && s[i].src_len) || (!s[i].dst && s[i].dst_cap) || s[i].format < 0 || s[i].format > 2)
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "stream %zu: bad descriptor", i);
-        in_off[i] = in_total;
-        out_off[i] = out_total;
-        in_total += align_up(s[i].src_len + 16, 256);
-        out_total += align_up(s[i].dst_cap + 16, 256);
+        in_off[i] = in.add(s[i].src_len);
+        out_off[i] = out.add(s[i].dst_cap);
     }
     if (memspace == PNGB200_MEM_HOST) {
-        CU(ctx->d_in.reserve(in_total));
-        CU(ctx->d_out.reserve(out_total));
+        CU(ctx->d_in.reserve(in.total));
+        CU(ctx->d_out.reserve(out.total));
         for (size_t i = 0; i < count; ++i)
             if (s[i].src_len)
                 CU(cudaMemcpyAsync(ctx->d_in.as<uint8_t>() + in_off[i], s[i].src, s[i].src_len,
@@ -1187,7 +1224,7 @@ int pngb200_decode_batch_enqueue(pngb200_ctx* ctx, pngb200_image_desc* im, size_
     ctx->expected.assign(count, 0);
     ctx->out_offset.assign(count, 0);
     ctx->out_bytes.assign(count, 0);
-    size_t f_total = 0, in_total = 0, out_total = 0;
+    Slots f{64}, in{16}, out{16};
     for (size_t i = 0; i < count; ++i) {
         if (!geometry(im[i].width, im[i].height, im[i].volume, im[i].depth, im[i].interlaced, &geo[i]) ||
             (!im[i].idat && im[i].idat_len) || !im[i].pixels || im[i].format > 1)
@@ -1196,22 +1233,19 @@ int pngb200_decode_batch_enqueue(pngb200_ctx* ctx, pngb200_image_desc* im, size_
             return set_error(ctx, PNGB200_ERR_OUTPUT_CAPACITY, "image %zu: pixels_cap %zu < %llu", i,
                              im[i].pixels_cap, (unsigned long long)geo[i].storage);
         ctx->expected[i] = geo[i].filtered;
-        f_off[i] = f_total;
-        f_total += align_up(geo[i].filtered + 64, 256);
-        in_off[i] = in_total;
-        in_total += align_up(im[i].idat_len + 16, 256);
-        ctx->out_offset[i] = out_total;
+        f_off[i] = f.add(geo[i].filtered);
+        in_off[i] = in.add(im[i].idat_len);
+        ctx->out_offset[i] = out.add(geo[i].storage);
         ctx->out_bytes[i] = geo[i].storage;
-        out_total += align_up(geo[i].storage + 16, 256);
     }
-    CU(ctx->d_filtered.reserve(f_total));
+    CU(ctx->d_filtered.reserve(f.total));
     CU(ctx->h_jobs.reserve(sizeof(StreamJob) * count));
     CU(ctx->d_jobs.reserve(sizeof(StreamJob) * count));
     CU(ctx->d_results.reserve(sizeof(StreamResult) * count));
     CU(ctx->h_results.reserve(sizeof(StreamResult) * count));
     if (host) {
-        CU(ctx->d_in.reserve(in_total));
-        CU(ctx->d_out.reserve(out_total));
+        CU(ctx->d_in.reserve(in.total));
+        CU(ctx->d_out.reserve(out.total));
         ctx->bulk_h2d = [ctx, im, count, &in_off]() -> int {  // runs inside run_inflate below, after its tables
             for (size_t i = 0; i < count; ++i)
                 if (im[i].idat_len)
@@ -1312,21 +1346,19 @@ int pngb200_unfilter_batch(pngb200_ctx* ctx, pngb200_image_desc* im, size_t coun
     const bool host = memspace == PNGB200_MEM_HOST;
     std::vector<UnfilterItem> items(count);
     std::vector<size_t>       f_off(count), o_off(count);
-    size_t f_total = 0, o_total = 0;
+    Slots f{64}, o{16};
     for (size_t i = 0; i < count; ++i) {
         UnfilterItem& it = items[i];
         if (!geometry(im[i].width, im[i].height, im[i].volume, im[i].depth, im[i].interlaced, &it.g) ||
             !im[i].idat || !im[i].pixels)
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: bad descriptor", i);
         if (im[i].pixels_cap < it.g.storage) return set_error(ctx, PNGB200_ERR_OUTPUT_CAPACITY, "image %zu: pixels_cap", i);
-        f_off[i] = f_total;
         // the generic kernel reconstructs in place, so it always works on a private copy
-        if (host || !it.g.fast) f_total += align_up(im[i].idat_len + 64, 256);
-        o_off[i] = o_total;
-        o_total += align_up(it.g.storage + 16, 256);
+        if (host || !it.g.fast) f_off[i] = f.add(im[i].idat_len);
+        o_off[i] = o.add(it.g.storage);
     }
-    CU(ctx->d_filtered.reserve(std::max<size_t>(f_total, 256)));
-    if (host) CU(ctx->d_out.reserve(o_total));
+    CU(ctx->d_filtered.reserve(std::max<size_t>(f.total, 256)));
+    if (host) CU(ctx->d_out.reserve(o.total));
     for (size_t i = 0; i < count; ++i) {
         UnfilterItem& it = items[i];
         uint8_t* priv = ctx->d_filtered.as<uint8_t>() + f_off[i];
@@ -1373,7 +1405,7 @@ int pngb200_filter_batch(pngb200_ctx* ctx, pngb200_filter_desc* im, size_t count
     const bool host = memspace == PNGB200_MEM_HOST;
     std::vector<FilterJob> jobs(count);
     std::vector<size_t>    p_off(count), f_off(count);
-    size_t p_total = 0, f_total = 0;
+    Slots p{16}, f{16};
     uint64_t rows = 0;
     std::vector<uint32_t> row_base(count + 1);
     for (size_t i = 0; i < count; ++i) {
@@ -1383,10 +1415,8 @@ int pngb200_filter_batch(pngb200_ctx* ctx, pngb200_filter_desc* im, size_t count
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: bad descriptor", i);
         if (im[i].pixels_len < g.storage || im[i].filtered_cap < g.filtered)
             return set_error(ctx, PNGB200_ERR_OUTPUT_CAPACITY, "image %zu: buffer too small", i);
-        p_off[i] = p_total;
-        f_off[i] = f_total;
-        p_total += align_up(g.storage + 16, 256);
-        f_total += align_up(g.filtered + 16, 256);
+        p_off[i] = p.add(g.storage);
+        f_off[i] = f.add(g.filtered);
         im[i].produced = g.filtered;
         row_base[i] = (uint32_t)rows;
         rows += filter_rows(im[i].width, im[i].height, im[i].interlaced);
@@ -1394,8 +1424,8 @@ int pngb200_filter_batch(pngb200_ctx* ctx, pngb200_filter_desc* im, size_t count
     row_base[count] = (uint32_t)rows;
     if (rows >= (1ull << 31)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
     if (host) {
-        CU(ctx->d_in.reserve(p_total));
-        CU(ctx->d_out.reserve(f_total));
+        CU(ctx->d_in.reserve(p.total));
+        CU(ctx->d_out.reserve(f.total));
         for (size_t i = 0; i < count; ++i)
             CU(cudaMemcpyAsync(ctx->d_in.as<uint8_t>() + p_off[i], im[i].pixels,
                                pngb200_storage_size(im[i].width, im[i].height, im[i].volume),
@@ -1411,17 +1441,12 @@ int pngb200_filter_batch(pngb200_ctx* ctx, pngb200_filter_desc* im, size_t count
         jobs[i].interlaced = im[i].interlaced;
         jobs[i].bpp = (uint8_t)((im[i].volume + 7) >> 3);
     }
-    size_t jb = sizeof(FilterJob) * count, rb = sizeof(uint32_t) * (count + 1);
-    size_t off_rb = align_up(jb, 256);
-    CU(ctx->h_genjobs.reserve(off_rb + rb));
-    CU(ctx->d_genjobs.reserve(off_rb + rb));
-    memcpy(ctx->h_genjobs.p, jobs.data(), jb);
-    memcpy((char*)ctx->h_genjobs.p + off_rb, row_base.data(), rb);
-    CU(cudaMemcpyAsync(ctx->d_genjobs.p, ctx->h_genjobs.p, off_rb + rb, cudaMemcpyHostToDevice, ctx->stream));
-    filter_rows_kernel<<<(unsigned)std::max<uint64_t>(1, (rows + FILTER_WARPS - 1) / FILTER_WARPS),
-                         FILTER_WARPS * 32, 0, ctx->stream>>>(
-        ctx->d_genjobs.as<FilterJob>(), (const uint32_t*)((char*)ctx->d_genjobs.p + off_rb),
-        (uint32_t)count, (uint32_t)rows);
+    Tables t(ctx->h_genjobs, ctx->d_genjobs);
+    const size_t off_jobs = t.host(jobs.data(), sizeof(FilterJob) * count);
+    const size_t off_rb = t.host(row_base.data(), sizeof(uint32_t) * (count + 1));
+    if (int rc = t.upload(ctx)) return rc;
+    filter_rows_kernel<<<(unsigned)std::max<uint64_t>(1, (rows + FILTER_WARPS - 1) / FILTER_WARPS), FILTER_WARPS * 32, 0, ctx->stream>>>(
+        t.dev<FilterJob>(off_jobs), t.dev<uint32_t>(off_rb), (uint32_t)count, (uint32_t)rows);
     ctx->launches++;
     CU(cudaGetLastError());
     if (host)
@@ -1539,26 +1564,21 @@ int run_color(pngb200_ctx* ctx, pngb200_color_desc* im, size_t count, int target
     std::vector<ColorJob> jobs(count);
     std::vector<size_t>   s_off(count), p_off(count), s_len(count);
     std::vector<uint32_t> palettes;
-    size_t s_total = 0, p_total = 0;
+    Slots st{16}, px{16};
     uint64_t most = 0;
     for (size_t i = 0; i < count; ++i) {
         const pngb200_pixel_format& f = im[i].format;
-        const int ch = f.color == 0 || f.color == 3 ? 1 : f.color == 2 ? 3 : f.color == 4 ? 2 : f.color == 6 ? 4 : 0;
-        const bool depth_ok = f.color == 3 ? (f.depth == 1 || f.depth == 2 || f.depth == 4 || f.depth == 8)
-                            : f.color == 0 ? (f.depth == 1 || f.depth == 2 || f.depth == 4 || f.depth == 8 || f.depth == 16)
-                                           : (f.depth == 8 || f.depth == 16);
-        if (!ch || !depth_ok || (f.bgr && (f.depth != 8 || (f.color != 2 && f.color != 6))) ||
-            (f.color == 3 && (!f.palette || f.palette_count == 0 || f.palette_count > 256)) ||
+        const PixelRule rule = pixel_rule(f.color, f.depth, f.bgr);
+        if (!rule.valid || (f.color == 3 && (!f.palette || f.palette_count == 0 || f.palette_count > 256)) ||
             (im[i].count && (!im[i].storage || !im[i].pixels)))
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: bad colour descriptor", i);
-        s_len[i] = (size_t)im[i].count * ch * (f.depth == 16 ? 2 : 1);
+        s_len[i] = (size_t)im[i].count * rule.channels * (f.depth == 16 ? 2 : 1);
         if (im[i].storage_len < s_len[i] || im[i].pixels_len < im[i].count * tpx)
             return set_error(ctx, PNGB200_ERR_OUTPUT_CAPACITY, "image %zu: buffer too small", i);
         if (!host && (((uintptr_t)im[i].pixels) & (std::min<size_t>(tpx, 16) - 1)))
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: pixel array is not aligned to its element size", i);
-        s_off[i] = s_total, p_off[i] = p_total;
-        s_total += align_up(s_len[i] + 16, 256);
-        p_total += align_up(im[i].count * tpx + 16, 256);
+        s_off[i] = st.add(s_len[i]);
+        p_off[i] = px.add(im[i].count * tpx);
         ColorJob& j = jobs[i];
         j.count = im[i].count;
         j.color = f.color, j.depth = f.depth, j.bgr = f.bgr, j.has_key = f.has_key;
@@ -1571,8 +1591,8 @@ int run_color(pngb200_ctx* ctx, pngb200_color_desc* im, size_t count, int target
         most = std::max<uint64_t>(most, im[i].count);
     }
     if (host) {
-        CU(ctx->d_in.reserve(unpack ? s_total : p_total));
-        CU(ctx->d_out.reserve(unpack ? p_total : s_total));
+        CU(ctx->d_in.reserve(unpack ? st.total : px.total));
+        CU(ctx->d_out.reserve(unpack ? px.total : st.total));
         for (size_t i = 0; i < count; ++i) {
             const size_t n = unpack ? s_len[i] : im[i].count * tpx;
             if (n)
@@ -1585,15 +1605,13 @@ int run_color(pngb200_ctx* ctx, pngb200_color_desc* im, size_t count, int target
         uint8_t* dev_p = host ? (unpack ? ctx->d_out : ctx->d_in).as<uint8_t>() + p_off[i] : (uint8_t*)im[i].pixels;
         jobs[i].storage = dev_s, jobs[i].pixels = dev_p;
     }
-    const size_t jb = sizeof(ColorJob) * count, off_pal = align_up(jb, 256), pb = sizeof(uint32_t) * std::max<size_t>(palettes.size(), 1);
-    CU(ctx->h_genjobs.reserve(off_pal + pb));
-    CU(ctx->d_genjobs.reserve(off_pal + pb));
-    memcpy(ctx->h_genjobs.p, jobs.data(), jb);
-    if (!palettes.empty()) memcpy((char*)ctx->h_genjobs.p + off_pal, palettes.data(), sizeof(uint32_t) * palettes.size());
-    CU(cudaMemcpyAsync(ctx->d_genjobs.p, ctx->h_genjobs.p, off_pal + pb, cudaMemcpyHostToDevice, ctx->stream));
+    Tables t(ctx->h_genjobs, ctx->d_genjobs);
+    const size_t jb = sizeof(ColorJob) * count, off_jobs = t.host(jobs.data(), jb);
+    const size_t off_pal = t.host(palettes.empty() ? nullptr : palettes.data(), sizeof(uint32_t) * std::max<size_t>(palettes.size(), 1));
+    if (int rc = t.upload(ctx)) return rc;
     ColorParams p;
-    p.jobs = ctx->d_genjobs.as<ColorJob>();
-    p.palettes = (const uint32_t*)((char*)ctx->d_genjobs.p + off_pal);
+    p.jobs = t.dev<ColorJob>(off_jobs);
+    p.palettes = t.dev<uint32_t>(off_pal);
     p.count = (uint32_t)count;
     p.target = target;
     p.alpha_mode = alpha_mode;
@@ -1625,9 +1643,9 @@ int run_color(pngb200_ctx* ctx, pngb200_color_desc* im, size_t count, int target
                 CU(cudaMemcpyAsync(unpack ? im[i].pixels : im[i].storage, ctx->d_out.as<uint8_t>() + (unpack ? p_off[i] : s_off[i]), n,
                                    cudaMemcpyDeviceToHost, ctx->stream));
         }
-    CU(cudaMemcpyAsync(ctx->h_genjobs.p, ctx->d_genjobs.p, jb, cudaMemcpyDeviceToHost, ctx->stream));
+    ColorJob* done = t.pin<ColorJob>(off_jobs);   // the jobs come back with their statuses
+    CU(cudaMemcpyAsync(done, t.dev<ColorJob>(off_jobs), jb, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
-    const ColorJob* done = ctx->h_genjobs.as<ColorJob>();
     for (size_t i = 0; i < count; ++i) im[i].status = done[i].status;
     return PNGB200_OK;
 }
@@ -1690,19 +1708,17 @@ extern "C" int pngb200_deflate_batch(pngb200_ctx* ctx, pngb200_deflate_desc* s, 
     const bool host = memspace == PNGB200_MEM_HOST;
     std::vector<DeflateJob> jobs(count);
     std::vector<size_t> in_off(count), out_off(count);
-    size_t in_total = 0, out_total = 0;
+    Slots in{16}, out{16};
     for (size_t i = 0; i < count; ++i) {
         if ((!s[i].src && s[i].src_len) || !s[i].dst || s[i].format < 0 || s[i].format > 2 || s[i].exponent < 8 ||
             s[i].exponent > 15)
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "stream %zu: bad descriptor", i);
-        in_off[i] = in_total;
-        out_off[i] = out_total;
-        in_total += align_up(s[i].src_len + 16, 256);
-        out_total += align_up(s[i].dst_cap + 16, 256);
+        in_off[i] = in.add(s[i].src_len);
+        out_off[i] = out.add(s[i].dst_cap);
     }
     if (host) {
-        CU(ctx->d_in.reserve(in_total));
-        CU(ctx->d_out.reserve(out_total));
+        CU(ctx->d_in.reserve(in.total));
+        CU(ctx->d_out.reserve(out.total));
         for (size_t i = 0; i < count; ++i)
             if (s[i].src_len)
                 CU(cudaMemcpyAsync(ctx->d_in.as<uint8_t>() + in_off[i], s[i].src, s[i].src_len,
@@ -1747,20 +1763,16 @@ extern "C" int pngb200_encode_batch(pngb200_ctx* ctx, pngb200_encode_desc* im, s
     // stage 1: filter into a private device workspace (device memspace of the filter entry point)
     std::vector<pngb200_filter_desc> fd(count);
     std::vector<size_t> f_off(count), p_off(count), o_off(count);
-    size_t f_total = 0, p_total = 0, o_total = 0;
+    Slots f{16}, p{16}, o{16};
     for (size_t i = 0; i < count; ++i) {
-        size_t fsz = pngb200_filtered_size(im[i].width, im[i].height, im[i].volume, im[i].interlaced);
-        f_off[i] = f_total;
-        f_total += align_up(fsz + 16, 256);
-        p_off[i] = p_total;
-        p_total += align_up(im[i].pixels_len + 16, 256);
-        o_off[i] = o_total;
-        o_total += align_up(im[i].idat_cap + 16, 256);
+        f_off[i] = f.add(pngb200_filtered_size(im[i].width, im[i].height, im[i].volume, im[i].interlaced));
+        p_off[i] = p.add(im[i].pixels_len);
+        o_off[i] = o.add(im[i].idat_cap);
     }
-    CU(ctx->d_enc.reserve(f_total + (host ? p_total + o_total : 0) + 256));
+    CU(ctx->d_enc.reserve(f.total + (host ? p.total + o.total : 0) + 256));
     uint8_t* d_f = ctx->d_enc.as<uint8_t>();
-    uint8_t* d_p = d_f + f_total;
-    uint8_t* d_o = d_p + (host ? p_total : 0);
+    uint8_t* d_p = d_f + f.total;
+    uint8_t* d_o = d_p + (host ? p.total : 0);
     for (size_t i = 0; i < count; ++i) {
         if (host) CU(cudaMemcpyAsync(d_p + p_off[i], im[i].pixels, im[i].pixels_len, cudaMemcpyHostToDevice, ctx->stream));
         fd[i].pixels = host ? d_p + p_off[i] : im[i].pixels;
@@ -1831,9 +1843,7 @@ void pngb200_inflator_destroy(pngb200_inflator* z)
     if (!z) return;
     DeviceGuard guard(z->ctx->device);
     cudaStreamSynchronize(z->ctx->stream);
-    for (DevBuf* b : {&z->d_in, &z->d_out, &z->d_job, &z->d_res, &z->d_misc, &z->d_partial}) b->release();
-    z->h_res.release();
-    delete z;
+    delete z;   // frees the workspaces
 }
 
 static int inflator_grow_out(pngb200_inflator* z, size_t need)
@@ -1845,12 +1855,8 @@ static int inflator_grow_out(pngb200_inflator* z, size_t need)
     cudaError_t e = cudaSuccess;
     if (z->produced) e = cudaMemcpyAsync(bigger.p, z->d_out.p, z->produced, cudaMemcpyDeviceToDevice, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) {
-        bigger.release();   // not adopted: give it back
-        return set_error(ctx, PNGB200_ERR_CUDA, "inflator: growing the output failed: %s", cudaGetErrorString(e));
-    }
-    z->d_out.release();
-    z->d_out = bigger;
+    if (e != cudaSuccess) return set_error(ctx, PNGB200_ERR_CUDA, "inflator: growing the output failed: %s", cudaGetErrorString(e));
+    z->d_out = std::move(bigger);   // the old output goes with `bigger`
     return PNGB200_OK;
 }
 
@@ -1866,8 +1872,7 @@ int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
     if (z->input.size() + 16 > z->d_in.cap) {
         DevBuf bigger;
         CU(bigger.reserve(z->input.size() * 2 + 4096));
-        z->d_in.release();
-        z->d_in = bigger;
+        z->d_in = std::move(bigger);   // the old copy goes with `bigger`
         z->uploaded = 0;
     }
     if (z->input.size() > z->uploaded)
@@ -1904,26 +1909,10 @@ int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
         // The stream checksum is only due when the trailer has been read: ONE pass over the output at the end of the
         // stream, not one per push (round 1 re-checksummed everything produced so far on every push).
         if (z->h_res.as<StreamResult>()->trailer_seen && !z->h_res.as<StreamResult>()->ck_done) {
-            uint32_t base[2] = {0, (uint32_t)((z->d_out.cap + CK_CHUNK - 1) / CK_CHUNK)};
-            CU(z->d_misc.reserve(sizeof base));
-            CU(z->d_partial.reserve(sizeof(uint64_t) * 2 * std::max<uint32_t>(base[1], 1)));
-            CU(cudaMemcpyAsync(z->d_misc.p, base, sizeof base, cudaMemcpyHostToDevice, ctx->stream));
-            ChecksumParams cp;
-            cp.jobs = z->d_job.as<StreamJob>();
-            cp.results = z->d_res.as<StreamResult>();
-            cp.chunk_base = z->d_misc.as<uint32_t>();
-            cp.partial = z->d_partial.as<uint64_t>();
-            cp.count = 1;
-            cp.total_chunks = base[1];
-            cp.crc_tables = nullptr;
-            if (z->format == PNGB200_FORMAT_GZIP) {
-                if (int rc = ensure_crc_tables(ctx)) return rc;
-                cp.crc_tables = ctx->d_crctab.as<uint32_t>();
-            }
-            checksum_chunk_kernel<<<base[1], CK_THREADS, 0, ctx->stream>>>(cp);
-            checksum_fold_kernel<<<1, 32, 0, ctx->stream>>>(cp);
-            ctx->launches += 2;
-            CU(cudaGetLastError());
+            // the inflator's own tables: it may run while a decode batch is pending on the context
+            uint32_t base[2];
+            rc = run_checksum(ctx, job, z->d_job.as<StreamJob>(), z->d_res.as<StreamResult>(), 1, base, z->d_misc, z->d_partial);
+            if (rc != PNGB200_OK) return rc;
             CU(cudaMemcpyAsync(z->h_res.p, z->d_res.p, sizeof(StreamResult), cudaMemcpyDeviceToHost, ctx->stream));
             CU(cudaStreamSynchronize(ctx->stream));
         }
