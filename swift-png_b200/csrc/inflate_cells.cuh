@@ -622,7 +622,8 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                     const uint64_t total64 = sh.warp_sums[WV_WARPS] & 0xffffffffffull;
                     const uint32_t np      = (uint32_t)(sh.warp_sums[WV_WARPS] >> 40);
                     const bool     cut     = total64 > CL_CAP;            // the wave is cut at the token that would overflow the cells
-                    if (sh.anomaly || out + total64 > job.dst_cap) {
+                    // (bit 1 only: a thread already in phase E may have set bit 2 for this wave -- read after barrier (7))
+                    if ((sh.anomaly & 1u) || out + total64 > job.dst_cap) {
                         S.fallback = true;
                         break;
                     }
@@ -665,7 +666,7 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                         piece(tok_walk + a_src * CL_WCAP, a_lo, a_hi);
                         piece(tok_mine, b_lo, b_hi);
                         piece(tok_walk + t * CL_WCAP, 0, c_hi);
-                        if (bad_ref) sh.anomaly = 1;
+                        if (bad_ref) sh.anomaly = 2;
                         from_staging = emitted;
 #ifdef PNGB200_EMU
                         if (!bad_ref && o != (uint32_t)o64 + my_nout) { fprintf(stderr, "cells: kept share of thread %u is %u bytes, expected %u\n", t, o - (uint32_t)o64, my_nout); abort(); }
@@ -691,7 +692,7 @@ __global__ void __launch_bounds__(WV_THREADS, CL_CTAS_PER_SM) inflate_cells_kern
                                 o += nb;
                                 ++emitted;
                             }
-                            if (bad_ref) sh.anomaly = 1;
+                            if (bad_ref) sh.anomaly = 2;
                         }
                     }
                     WV_COUNT(2, emitted);

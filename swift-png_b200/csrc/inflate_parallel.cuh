@@ -338,7 +338,8 @@ __device__ __forceinline__ void inflate_parallel_body(WvParams P)
                     uint32_t       c_next  = (uint32_t)(excl >> 40);           // my first list slot
                     const uint32_t total   = (uint32_t)(sh.warp_sums[PAR_WARPS] & 0xffffffffffull);
                     const uint32_t np      = (uint32_t)(sh.warp_sums[PAR_WARPS] >> 40);
-                    if (sh.anomaly || out + total > job.dst_cap || total > P.bitmap_words * 32) {
+                    // (bit 1 only: a thread already emitting may have set bit 2 for this wave -- read after the next barrier)
+                    if ((sh.anomaly & 1u) || out + total > job.dst_cap || total > P.bitmap_words * 32) {
                         fallback = true;
                         break;
                     }
@@ -381,7 +382,7 @@ __device__ __forceinline__ void inflate_parallel_body(WvParams P)
                                 continue;
                             }
                             if ((uint64_t)dist > out + o) {  // invalidStringReference
-                                sh.anomaly = 1;
+                                sh.anomaly = 2;
                                 break;
                             }
                             // flag [o, o + run) as unresolved; words are flushed once, when left

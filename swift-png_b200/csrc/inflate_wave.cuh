@@ -554,7 +554,8 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                     const uint32_t c_start = (uint32_t)(excl >> 40);           // my first list slot
                     const uint64_t total64 = sh.warp_sums[WV_WARPS] & 0xffffffffffull;
                     const uint32_t np      = (uint32_t)(sh.warp_sums[WV_WARPS] >> 40);
-                    if (sh.anomaly || out + total64 > dst_cap || total64 > P.bitmap_words * 32) {
+                    // (bit 1 only: a thread already in phase E may have set bit 2 for this wave -- read after barrier (7))
+                    if ((sh.anomaly & 1u) || out + total64 > dst_cap || total64 > P.bitmap_words * 32) {
                         S.fallback = true;
                         over_cap = out + total64 > dst_cap;
                         break;
@@ -605,7 +606,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                                 ++emitted;
                             }
                         }
-                        if (S.bad_ref) sh.anomaly = 1;
+                        if (S.bad_ref) sh.anomaly = 2;
                         deferred = S.c_next - c_start;
                     }
                     WV_COUNT(2, emitted);
