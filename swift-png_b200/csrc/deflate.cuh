@@ -125,6 +125,7 @@ __device__ int df_heap_lowest(DfShared& S, int count, int parent)
 }
 __device__ void df_heap_swap(DfShared& S, int i, int j)
 {
+    __syncwarp();   // every lane has read the keys (df_heap_lowest, df_sift_up, the dequeue) before lane 0 moves them
     if (lane_id() == 0) {
         uint32_t k = S.hkey[i - 1]; S.hkey[i - 1] = S.hkey[j - 1]; S.hkey[j - 1] = k;
         uint16_t d = S.hid[i - 1]; S.hid[i - 1] = S.hid[j - 1]; S.hid[j - 1] = d;
@@ -799,7 +800,7 @@ __device__ int df_write_block(DfState& z, DfShared& S, DfOut& out, bool final)
 
 __global__ void __launch_bounds__(32) deflate_kernel(DfParams P)
 {
-    extern __shared__ __align__(16) unsigned char df_smem[];
+    PNGB200_DYN_SMEM(df_smem);
     DfShared& S = *reinterpret_cast<DfShared*>(df_smem);
     const unsigned lane = lane_id();
     uint8_t* slot = P.scratch + blockIdx.x * P.scratch_stride;
