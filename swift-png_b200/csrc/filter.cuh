@@ -20,7 +20,8 @@ struct FilterJob {
     uint8_t        volume, depth, interlaced, bpp;
 };
 
-constexpr int FILTER_WARPS = 8;
+constexpr int      FILTER_WARPS = 8;
+constexpr uint32_t FILTER_SLICE = 1u << 29;   // bytes of a row a warp scores in 32-bit lane sums (see filter_rows_kernel)
 
 inline uint64_t filter_rows(uint32_t w, uint32_t h, int interlaced)
 {
@@ -108,31 +109,41 @@ filter_rows_kernel(const FilterJob* jobs, const uint32_t* row_base, uint32_t njo
     prev.oy = by + ((y ? y - 1 : 0) << ey);
     const uint32_t d = job.bpp;
 
-    uint32_t s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0;
-    for (uint32_t i = lane; i < pitch; i += 32) {
-        uint32_t x = cur.byte(i), b = prev.byte(i);
-        uint32_t a = i >= d ? cur.byte(i - d) : 0, c = i >= d ? prev.byte(i - d) : 0;
-        s0 += abs_i8(x);
-        s1 += abs_i8((x - a) & 0xff);
-        s2 += abs_i8((x - b) & 0xff);
-        s3 += abs_i8((x - ((a + b) >> 1)) & 0xff);
-        s4 += abs_i8((x - paeth1(a, b, c)) & 0xff);
+    // A row scores up to 128 * pitch, past 2^32 from pitch 2^25 on (the reference sums in Swift Int): the scores are
+    // 64-bit.  Each lane sums a slice of FILTER_SLICE bytes in 32 bits (at most FILTER_SLICE / 32 * 128 = 2^31) and
+    // folds it into its 64-bit totals; slice offsets also keep the byte index from wrapping on a 4 GiB row.
+    uint64_t t0 = 0, t1 = 0, t2 = 0, t3 = 0, t4 = 0;
+    for (uint64_t base = 0; base < pitch; base += FILTER_SLICE) {
+        const uint32_t n = (uint32_t)min((uint64_t)FILTER_SLICE, pitch - base);
+        uint32_t s0 = 0, s1 = 0, s2 = 0, s3 = 0, s4 = 0;
+        for (uint32_t k = lane; k < n; k += 32) {
+            const uint32_t i = (uint32_t)base + k;
+            uint32_t x = cur.byte(i), b = prev.byte(i);
+            uint32_t a = i >= d ? cur.byte(i - d) : 0, c = i >= d ? prev.byte(i - d) : 0;
+            s0 += abs_i8(x);
+            s1 += abs_i8((x - a) & 0xff);
+            s2 += abs_i8((x - b) & 0xff);
+            s3 += abs_i8((x - ((a + b) >> 1)) & 0xff);
+            s4 += abs_i8((x - paeth1(a, b, c)) & 0xff);
+        }
+        t0 += s0; t1 += s1; t2 += s2; t3 += s3; t4 += s4;
     }
     for (int o = 16; o; o >>= 1) {
-        s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-        s3 += __shfl_xor_sync(0xffffffffu, s3, o);
-        s4 += __shfl_xor_sync(0xffffffffu, s4, o);
+        t0 += __shfl_xor_sync(0xffffffffu, t0, o);
+        t1 += __shfl_xor_sync(0xffffffffu, t1, o);
+        t2 += __shfl_xor_sync(0xffffffffu, t2, o);
+        t3 += __shfl_xor_sync(0xffffffffu, t3, o);
+        t4 += __shfl_xor_sync(0xffffffffu, t4, o);
     }
-    uint32_t best = 0, minimum = s0;
-    if (s1 < minimum) { minimum = s1; best = 1; }
-    if (s2 < minimum) { minimum = s2; best = 2; }
-    if (s3 < minimum) { minimum = s3; best = 3; }
-    if (s4 < minimum) { minimum = s4; best = 4; }
+    uint32_t best = 0;
+    uint64_t minimum = t0;
+    if (t1 < minimum) { minimum = t1; best = 1; }
+    if (t2 < minimum) { minimum = t2; best = 2; }
+    if (t3 < minimum) { minimum = t3; best = 3; }
+    if (t4 < minimum) { minimum = t4; best = 4; }
     uint8_t* out = job.filtered + out_off;
     if (lane == 0) out[0] = (uint8_t)best;
-    for (uint32_t i = lane; i < pitch; i += 32) {
+    for (uint64_t i = lane; i < pitch; i += 32) {
         uint32_t x = cur.byte(i), p = 0;
         if (best) {
             uint32_t b = prev.byte(i);

@@ -187,7 +187,7 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
     const uint8_t* in    = row + 1;
     const uint32_t m     = (uint32_t)((uintptr_t)in & 15);
     const uint4*   inq   = (const uint4*)(in - m);
-    const int      nq    = (int)((m + pitch + 15) >> 4);  // aligned chunks that hold row bytes
+    const int      nq    = (int)(((uint64_t)m + pitch + 15) >> 4);  // aligned chunks that hold row bytes
     uint8_t*       out   = job.pixels + (uint64_t)(active ? y : 0) * pitch;
     const uint8_t* above = band == 0 ? nullptr : job.pixels + (uint64_t)(band * 32 - 1) * pitch;
     const bool     publish = lane == 31 && prog_mine != nullptr;
@@ -300,7 +300,8 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
                 held = o;
             } else {
                 if (j & 1) store16_partial(out + 16 * (uint64_t)(j - 1), held, 16);
-                store16_partial(out + 16 * (uint64_t)j, o, (int)pitch - 16 * j);
+                // bytes of the row from chunk j on, capped at 16 before the narrowing: pitch can pass 2^31
+                store16_partial(out + 16 * (uint64_t)j, o, (int)min(pitch - 16u * (uint32_t)j, 16u));
             }
             mine = o;
             if (publish && (((j + 1) % WAVE_PUBLISH) == 0 || j + 1 == nchunk)) {
@@ -398,7 +399,9 @@ __global__ void __launch_bounds__(128) unfilter_generic_kernel(const GenericJob*
             shh = (job.height + (1u << ey) - by - 1) >> ey;
             if (sw == 0 || shh == 0) continue;
         }
-        const uint32_t pitch = (sw * job.volume + 7) >> 3;
+        // sw * volume passes 2^32 from sw = 2^26 (RGBA16) on: the pitch is computed in 64 bits (it fits 32 again, as
+        // geometry() caps it at 0xfffffff0), and the byte loops below count in 64 bits so that i + nt cannot wrap
+        const uint32_t pitch = (uint32_t)(((uint64_t)sw * job.volume + 7) >> 3);
         uint8_t*       last  = nullptr;
         for (uint32_t y = 0; y < shh; ++y) {
             if (at + pitch + 1 > end) return;  // inflator.pull(pitch + 1) == nil
@@ -406,10 +409,10 @@ __global__ void __launch_bounds__(128) unfilter_generic_kernel(const GenericJob*
             const uint8_t type = at[0];
             if (type == 2) {
                 if (last)
-                    for (uint32_t i = tid; i < pitch; i += nt) line[i] = (uint8_t)(line[i] + last[i]);
+                    for (uint64_t i = tid; i < pitch; i += nt) line[i] = (uint8_t)(line[i] + last[i]);
             } else if (type == 1 || type == 3 || type == 4) {
                 if ((uint32_t)tid < bpp) {  // channels are independent chains
-                    for (uint32_t i = tid; i < pitch; i += bpp) {
+                    for (uint64_t i = tid; i < pitch; i += bpp) {
                         uint32_t a = i >= bpp ? line[i - bpp] : 0;
                         uint32_t b = last ? last[i] : 0;
                         uint32_t c = (last && i >= bpp) ? last[i - bpp] : 0;
@@ -429,8 +432,8 @@ __global__ void __launch_bounds__(128) unfilter_generic_kernel(const GenericJob*
                         (uint8_t)((line[i / per] >> sh) & mask);
                 }
             } else {
-                for (uint32_t k = tid; k < sw * bpp; k += nt) {
-                    uint32_t i = k / bpp, c = k - i * bpp;
+                for (uint64_t k = tid; k < pitch; k += nt) {   // depth >= 8: sw * bpp == pitch
+                    uint32_t i = (uint32_t)k / bpp, c = (uint32_t)k - i * bpp;
                     job.pixels[((uint64_t)oy * job.width + bx + ((uint64_t)i << ex)) * bpp + c] = line[k];
                 }
             }
