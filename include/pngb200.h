@@ -337,7 +337,7 @@ int pngb200_encode_batch(pngb200_ctx* ctx, pngb200_encode_desc* images, size_t c
  * other than PLTE / tRNS / bKGD are CRC-checked and otherwise ignored (metadata is not on the hot path).
  * Errors come back in the order the reference's streaming loop meets them. */
 typedef struct pngb200_png_desc {
-    const uint8_t*       file;          /* in: the PNG file, HOST memory */
+    const uint8_t*       file;          /* in: the PNG file, HOST memory (pngb200_png_*_files: file_memspace) */
     size_t               file_len;
     void*                pixels;        /* out: PNG.Image.storage (memspace of the call) */
     size_t               pixels_cap;    /* >= storage_size (pngb200_png_inspect_batch reports it) */
@@ -355,10 +355,23 @@ typedef struct pngb200_png_desc {
     uint64_t             produced;
 } pngb200_png_desc;
 /* host only: walk the chunk headers, parse IHDR / PLTE / tRNS, fill the out fields (no CRC check, no
- * GPU) -- what a caller needs to size `pixels` */
+ * GPU) -- what a caller needs to size `pixels`.  pngb200_png_inspect_files(NULL, files, count, PNGB200_MEM_HOST). */
 int pngb200_png_inspect_batch(pngb200_png_desc* files, size_t count);
-/* `memspace` is where `pixels` live; files are always host memory */
+/* `memspace` is where `pixels` live; files are host memory.
+ * pngb200_png_decode_files(ctx, files, count, PNGB200_MEM_HOST, memspace). */
 int pngb200_png_decode_batch(pngb200_ctx* ctx, pngb200_png_desc* files, size_t count, int memspace);
+
+/* The same calls for files anywhere.  file_memspace: where every `file` points (PNGB200_MEM_DEVICE: the context's
+ * GPU, any alignment); memspace: where `pixels` live, as in pngb200_png_decode_batch.  Every out field, every pixel
+ * and every error is what the host-file calls give for the same bytes.
+ * With device files the chunk walk runs on the GPU (one warp per file; inside an IDAT run the warp checks 32 chunk
+ * headers a step) and the host receives a small summary per file and the chunk records; CRC-32 regions point into
+ * the files themselves, and the IDAT run is gathered device to device into the context's payload arena, so the
+ * decoder never reads a caller pointer.  A device-file batch runs as one piece on the context (there is no host copy
+ * to overlap).  pngb200_png_inspect_files needs `ctx` only for device files; it does not check CRCs.
+ * A file_memspace other than HOST or DEVICE, or a call while a decode batch is pending: PNGB200_ERR_BAD_ARGUMENT. */
+int pngb200_png_inspect_files(pngb200_ctx* ctx, pngb200_png_desc* files, size_t count, int file_memspace);
+int pngb200_png_decode_files(pngb200_ctx* ctx, pngb200_png_desc* files, size_t count, int file_memspace, int memspace);
 
 typedef struct pngb200_png_encode_desc {
     const void*          pixels;        /* in: PNG.Image.storage (memspace of the call) */
@@ -369,7 +382,7 @@ typedef struct pngb200_png_encode_desc {
     int32_t              level;         /* 0...13 */
     uint32_t             idat_chunk;    /* bytes per IDAT chunk; 0 = 65544, what the reference emits for its
                                            default hint (2 x the capacity malloc gives DeflatorOut's buffer) */
-    uint8_t*             file;          /* out: the PNG file, HOST memory */
+    uint8_t*             file;          /* out: the PNG file, HOST memory (pngb200_png_encode_files: file_memspace) */
     size_t               file_cap;      /* >= pngb200_png_encode_bound(...) */
     int32_t              status;
     uint32_t             checksum, blocks;
@@ -378,6 +391,12 @@ typedef struct pngb200_png_encode_desc {
 size_t pngb200_png_encode_bound(uint32_t width, uint32_t height, const pngb200_pixel_format* format, int interlaced,
                                 uint32_t idat_chunk);
 int    pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* images, size_t count, int memspace);
+/* pngb200_png_encode_batch for files anywhere: with file_memspace PNGB200_MEM_DEVICE, `file` is a device buffer on
+ * the context's GPU and the file is written straight into it (head by one small host-to-device copy, IDAT framing and
+ * CRC-32 in place, IEND) -- the same bytes pngb200_png_encode_batch writes, with no device-to-host copy.  file_cap and
+ * pngb200_png_encode_bound are unchanged.  A file_memspace other than HOST or DEVICE: PNGB200_ERR_BAD_ARGUMENT. */
+int    pngb200_png_encode_files(pngb200_ctx* ctx, pngb200_png_encode_desc* images, size_t count, int memspace,
+                                int file_memspace);
 
 /* size helpers (host arithmetic only) */
 size_t pngb200_filtered_size(uint32_t width, uint32_t height, int volume, int interlaced);

@@ -212,6 +212,12 @@ def lib():
     L.pngb200_png_encode_bound.restype = C.c_size_t
     L.pngb200_png_encode_batch.argtypes = [C.c_void_p, C.POINTER(PngEncodeDesc), C.c_size_t, C.c_int]
     L.pngb200_png_encode_batch.restype = C.c_int
+    L.pngb200_png_inspect_files.argtypes = [C.c_void_p, C.POINTER(PngDesc), C.c_size_t, C.c_int]
+    L.pngb200_png_inspect_files.restype = C.c_int
+    L.pngb200_png_decode_files.argtypes = [C.c_void_p, C.POINTER(PngDesc), C.c_size_t, C.c_int, C.c_int]
+    L.pngb200_png_decode_files.restype = C.c_int
+    L.pngb200_png_encode_files.argtypes = [C.c_void_p, C.POINTER(PngEncodeDesc), C.c_size_t, C.c_int, C.c_int]
+    L.pngb200_png_encode_files.restype = C.c_int
     L.pngb200_ctx_trim.argtypes = [C.c_void_p]
     L.pngb200_ctx_trim.restype = C.c_int
     L.pngb200_last_error.argtypes = [C.c_void_p]
@@ -643,6 +649,73 @@ def png_encode_batch(ctx: Context, images, level: int = 9, idat_chunk: int = 0):
     ctx.check(ctx._lib.pngb200_png_encode_batch(ctx.handle, descs, n, MEM_HOST))
     pairs = [k for k in keep if isinstance(k, tuple)]
     return [(descs[i].status, pairs[i][1].raw[: descs[i].produced]) for i in range(n)]
+
+
+def _device_png_descs(files):
+    """descriptors for PNG files in device memory: `files` are (address, length) pairs"""
+    files = [(int(a or 0), int(n)) for a, n in files]
+    descs = (PngDesc * max(len(files), 1))()
+    for i, (a, n) in enumerate(files):
+        descs[i].file, descs[i].file_len = a or None, n
+    return descs, len(files)
+
+
+def png_inspect_files(ctx: Context, files):
+    """pngb200_png_inspect_files over device files, (address, length) pairs: the chunk walk on the GPU (no CRC
+    check).  Returns [PngImage]."""
+    descs, n = _device_png_descs(files)
+    ctx.check(ctx._lib.pngb200_png_inspect_files(ctx.handle, descs, n, MEM_DEVICE))
+    return [PngImage(descs[i], None) for i in range(n)]
+
+
+def png_decode_files(ctx: Context, files, pixels=None):
+    """PNG.Image.decompress(stream:) over PNG files already in device memory, (address, length) pairs.  pixels=None:
+    storage comes back as bytes, as from png_decode_batch; else (address, capacity) device buffers, one per file,
+    that receive it (PngImage.storage is then None).  Returns [PngImage]."""
+    descs, n = _device_png_descs(files)
+    ctx.check(ctx._lib.pngb200_png_inspect_files(ctx.handle, descs, n, MEM_DEVICE))
+    outs = []
+    for i in range(n):
+        if pixels is None:
+            dst = C.create_string_buffer(max(int(descs[i].storage_size), 1))
+            outs.append(dst)
+            descs[i].pixels, descs[i].pixels_cap = _buf_addr(dst), int(descs[i].storage_size)
+        else:
+            descs[i].pixels, descs[i].pixels_cap = int(pixels[i][0]) or None, int(pixels[i][1])
+    memspace = MEM_HOST if pixels is None else MEM_DEVICE
+    ctx.check(ctx._lib.pngb200_png_decode_files(ctx.handle, descs, n, MEM_DEVICE, memspace))
+    return [PngImage(descs[i], outs[i].raw[: descs[i].storage_size] if pixels is None and descs[i].status == OK else None)
+            for i in range(n)]
+
+
+def png_encode_bound(image, idat_chunk: int = 0) -> int:
+    """pngb200_png_encode_bound for one png_encode_batch image dict: the file capacity to provide"""
+    f, keep = PixelFormat(), []
+    _fill_format(f, keep, image["color"], image["depth"], image.get("bgr"), image.get("key"), image.get("palette"))
+    return lib().pngb200_png_encode_bound(image["width"], image["height"], C.byref(f),
+                                          int(bool(image.get("interlaced", False))), idat_chunk)
+
+
+def png_encode_files(ctx: Context, images, files, level: int = 9, idat_chunk: int = 0):
+    """PNG.Image.compress(stream:level:) over a batch, each file written straight into a device buffer: images as for
+    png_encode_batch, files (address, capacity) pairs of at least png_encode_bound bytes.  Returns [(status, file
+    bytes written)]."""
+    images = list(images)
+    n = len(images)
+    descs = (PngEncodeDesc * max(n, 1))()
+    keep = []
+    for i, g in enumerate(images):
+        st = bytes(g["storage"])
+        src = C.create_string_buffer(st, len(st))
+        keep.append(src)
+        _fill_format(descs[i].format, keep, g["color"], g["depth"], g.get("bgr"), g.get("key"), g.get("palette"))
+        descs[i].pixels, descs[i].pixels_len = _buf_addr(src), len(st)
+        descs[i].width, descs[i].height, descs[i].interlaced = g["width"], g["height"], int(bool(g.get("interlaced", False)))
+        descs[i].level = level if isinstance(level, int) else level[i]
+        descs[i].idat_chunk = idat_chunk
+        descs[i].file, descs[i].file_cap = int(files[i][0]) or None, int(files[i][1])
+    ctx.check(ctx._lib.pngb200_png_encode_files(ctx.handle, descs, n, MEM_HOST, MEM_DEVICE))
+    return [(descs[i].status, int(descs[i].produced)) for i in range(n)]
 
 
 def deflate_batch(ctx: Context, streams, level: int = 9, fmt: int = FORMAT_ZLIB, exponent: int = 15):

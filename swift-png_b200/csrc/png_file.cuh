@@ -8,51 +8,17 @@
 // segment_copy_kernel concatenates IDAT bodies when a file has more than one, and the batch decode
 // path runs on the result.  Errors are reported in the order the reference's streaming loop would
 // meet them (see resolve order below).  Encode mirrors compress(stream:level:hint:) (:576-670).
+// Files already in device memory take the same path with the walk on the device (png_walk.cuh): nothing is staged
+// but the gathered IDAT run, and an encoded file is written where the caller wants it.
 #pragma once
 
 namespace {
 
-constexpr uint32_t fourcc(char a, char b, char c, char d)
-{
-    return (uint32_t)(uint8_t)a << 24 | (uint32_t)(uint8_t)b << 16 | (uint32_t)(uint8_t)c << 8 | (uint32_t)(uint8_t)d;
-}
-constexpr uint32_t CK_CgBI = fourcc('C', 'g', 'B', 'I'), CK_IHDR = fourcc('I', 'H', 'D', 'R'), CK_PLTE = fourcc('P', 'L', 'T', 'E'),
-                   CK_IDAT = fourcc('I', 'D', 'A', 'T'), CK_IEND = fourcc('I', 'E', 'N', 'D'), CK_tRNS = fourcc('t', 'R', 'N', 'S'),
-                   CK_bKGD = fourcc('b', 'K', 'G', 'D'), CK_hIST = fourcc('h', 'I', 'S', 'T'), CK_cHRM = fourcc('c', 'H', 'R', 'M'),
-                   CK_gAMA = fourcc('g', 'A', 'M', 'A'), CK_sRGB = fourcc('s', 'R', 'G', 'B'), CK_iCCP = fourcc('i', 'C', 'C', 'P'),
-                   CK_sBIT = fourcc('s', 'B', 'I', 'T'), CK_pHYs = fourcc('p', 'H', 'Y', 's'), CK_sPLT = fourcc('s', 'P', 'L', 'T'),
-                   CK_tIME = fourcc('t', 'I', 'M', 'E'), CK_iTXt = fourcc('i', 'T', 'X', 't'), CK_tEXt = fourcc('t', 'E', 'X', 't'),
-                   CK_zTXt = fourcc('z', 'T', 'X', 't');
 const uint8_t PNG_SIGNATURE[8] = {137, 80, 78, 71, 13, 10, 26, 10};
 
-inline uint32_t load_be32(const uint8_t* p) { return (uint32_t)p[0] << 24 | (uint32_t)p[1] << 16 | (uint32_t)p[2] << 8 | p[3]; }
-inline uint32_t load_be16(const uint8_t* p) { return (uint32_t)p[0] << 8 | p[1]; }
-inline void     store_be32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)(v >> 24), p[1] = (uint8_t)(v >> 16), p[2] = (uint8_t)(v >> 8), p[3] = (uint8_t)v; }
+inline void store_be32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)(v >> 24), p[1] = (uint8_t)(v >> 16), p[2] = (uint8_t)(v >> 8), p[3] = (uint8_t)v; }
 
-// PNG.Chunk.init(validating:) (Lexing/PNG.Chunk.swift:39-58)
-inline bool chunk_type_ok(uint32_t name)
-{
-    switch (name) {
-    case CK_CgBI: case CK_IHDR: case CK_PLTE: case CK_IDAT: case CK_IEND: case CK_cHRM: case CK_gAMA: case CK_iCCP:
-    case CK_sBIT: case CK_sRGB: case CK_bKGD: case CK_hIST: case CK_tRNS: case CK_pHYs: case CK_sPLT: case CK_tIME:
-    case CK_iTXt: case CK_tEXt: case CK_zTXt:
-        return true;
-    default:
-        return (name & 0x20002000u) == 0x20000000u;
-    }
-}
-
-struct ChunkRec {
-    uint64_t off;       // offset of the chunk's length field in the file
-    uint32_t len;       // body bytes
-    uint32_t type;
-    uint32_t declared;  // CRC-32 stored behind the body
-};
-
-// What the header walk learned about one file.  `stop` is the index of the chunk at which the
-// reference would have thrown for a structural reason (chunks.size() if none); `stop_before_crc`
-// tells whether that happens before the chunk's own CRC check (lexing) or after it (parsing /
-// ordering).
+// What the chunk walk (png_walk.cuh) learned about one file, with every lexed chunk's record
 struct FileWalk {
     std::vector<ChunkRec> chunks;
     int      status = PNGB200_OK;
@@ -62,151 +28,86 @@ struct FileWalk {
     size_t   first_idat = (size_t)-1, idat_end = 0;  // [first_idat, idat_end): the contiguous IDAT run
 };
 
-// Walks the chunk headers of one file and parses IHDR / PLTE / tRNS into `d`
-// (PNG.Image.decompress(stream:), PNG.Image.swift:298-401; PNG.Header.init(parsing:standard:),
-// Parsing/PNG.Header.swift:40-98; PNG.Palette.init(parsing:pixel:), PNG.Palette.swift:27-55;
-// PNG.Transparency.init(parsing:pixel:palette:), PNG.Transparency.swift:68-122; ordering rules of
-// Decoding/PNG.Metadata.swift:70-92 and PNG.Context.swift:51-81).  No payload byte other than those
-// three chunks' is read.
+// the out fields of `d` and the scalars of `w` from a walk's summary; `palette`: the palette the walk wrote, null when
+// it wrote into d.palette_rgba itself
+void take_walk(const WalkHead& h, const uint8_t* palette, pngb200_png_desc& d, FileWalk& w)
+{
+    d.width = h.width, d.height = h.height;
+    d.depth = h.depth, d.color = h.color, d.interlaced = h.interlaced, d.standard = h.standard;
+    d.format = h.format;
+    d.format.palette = d.palette_rgba;
+    if (palette) memcpy(d.palette_rgba, palette, 4 * (size_t)h.palette_entries);
+    d.storage_size = h.storage_size, d.idat_bytes = h.idat_bytes;
+    d.idat_chunks = h.idat_chunks, d.chunks = (uint32_t)h.chunks;
+    w.status = h.status, w.a = h.a, w.b = h.b;
+    w.stop = (size_t)h.stop, w.stop_before_crc = h.stop_before_crc != 0;
+    w.first_idat = (size_t)h.first_idat, w.idat_end = (size_t)h.idat_end;
+}
+
+struct RecordVector {
+    std::vector<ChunkRec>* v;
+    void put(uint64_t, const ChunkRec& r) const { v->push_back(r); }
+};
+
+// the walk of a host file, on the host
 void walk_file(pngb200_png_desc& d, FileWalk& w)
 {
-    const uint8_t* f = d.file;
-    const size_t   n = d.file_len;
-    auto stop = [&](int status, uint32_t a, uint32_t b, bool before_crc) {
-        w.status = status, w.a = a, w.b = b;
-        w.stop = w.chunks.size() - (before_crc ? 0 : 1);
-        w.stop_before_crc = before_crc;
-    };
-    d.width = d.height = 0;
-    d.depth = d.color = d.interlaced = d.standard = 0;
-    memset(&d.format, 0, sizeof d.format);
-    d.format.palette = d.palette_rgba;
-    d.storage_size = d.idat_bytes = 0;
-    d.idat_chunks = d.chunks = 0;
-    if (n < 8) { w.status = PNGB200_ERR_LEX_TRUNCATED_SIGNATURE, w.stop = 0, w.stop_before_crc = true; return; }
-    if (memcmp(f, PNG_SIGNATURE, 8)) {
-        w.status = PNGB200_ERR_LEX_INVALID_SIGNATURE, w.a = load_be32(f), w.b = load_be32(f + 4), w.stop = 0, w.stop_before_crc = true;
-        return;
+    WalkHead h;
+    w.chunks.clear();
+    walk_png<false>(d.file, d.file_len, h, d.palette_rgba, RecordVector{&w.chunks}, true);
+    take_walk(h, nullptr, d, w);
+}
+
+// The walk of device files, on the device (png_walk_kernel): pass 1 fills the out fields of `d` and the scalars of
+// `walks`; with `records`, pass 2 brings every chunk's record back too (24 bytes a chunk), into record arrays sized
+// from pass 1's counts.  The summaries and records pass through the file arena, which a device-file batch does not
+// otherwise use.
+int walk_device_files(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, std::vector<FileWalk>& walks, bool records)
+{
+    std::vector<WalkFile> files(count);
+    for (size_t i = 0; i < count; ++i) {
+        if (!d[i].file && d[i].file_len) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "file %zu: null pointer", i);
+        files[i] = {d[i].file, d[i].file_len};
     }
-    size_t at = 8;
-    // lexes one chunk header; false = stopped
-    auto lex = [&]() -> bool {
-        if (n - at < 8) { stop(PNGB200_ERR_LEX_TRUNCATED_CHUNK_HEADER, 0, 0, true); return false; }
-        const uint32_t len = load_be32(f + at), name = load_be32(f + at + 4);
-        if (!chunk_type_ok(name)) { stop(PNGB200_ERR_LEX_INVALID_CHUNK_TYPE, name, 0, true); return false; }
-        if ((uint64_t)(n - at - 8) < (uint64_t)len + 4) { stop(PNGB200_ERR_LEX_TRUNCATED_CHUNK_BODY, len + 4, 0, true); return false; }
-        w.chunks.push_back({at, len, name, load_be32(f + at + 8 + len)});
-        at += 12 + (size_t)len;
-        return true;
-    };
-    if (!lex()) return;
-    if (w.chunks.back().type == CK_CgBI) {
-        d.standard = 1;
-        if (!lex()) return;
-    }
+    if (count == 0) return PNGB200_OK;
+    if (count > 0xffffffffu) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
+    const unsigned grid = (unsigned)((count + WALK_WARPS - 1) / WALK_WARPS);
+    const size_t   sum_bytes = sizeof(WalkSummary) * count;
+    std::vector<uint64_t> base(count + 1, 0);
     {
-        const ChunkRec& c = w.chunks.back();
-        if (c.type != CK_IHDR) return stop(PNGB200_ERR_DECODE_REQUIRED_CHUNK, CK_IHDR, c.type, false);
-        const uint8_t* h = f + c.off + 8;
-        if (c.len != 13) return stop(PNGB200_ERR_PARSE_HEADER_CHUNK_LENGTH, c.len, 0, false);
-        const int depth = h[8], color = h[9];
-        const PixelRule rule = pixel_rule(color, depth, false);
-        if (!rule.valid) return stop(PNGB200_ERR_PARSE_HEADER_PIXEL_FORMAT_CODE, (uint32_t)depth, (uint32_t)color, false);
-        if (d.standard == 1 && !pixel_rule(color, depth, true).valid)
-            return stop(PNGB200_ERR_PARSE_HEADER_PIXEL_FORMAT, (uint32_t)depth, (uint32_t)color, false);
-        if (h[10]) return stop(PNGB200_ERR_PARSE_HEADER_COMPRESSION_CODE, h[10], 0, false);
-        if (h[11]) return stop(PNGB200_ERR_PARSE_HEADER_FILTER_CODE, h[11], 0, false);
-        if (h[12] > 1) return stop(PNGB200_ERR_PARSE_HEADER_INTERLACING_CODE, h[12], 0, false);
-        d.width = load_be32(h), d.height = load_be32(h + 4);
-        if (!d.width || !d.height) return stop(PNGB200_ERR_PARSE_HEADER_SIZE, d.width, d.height, false);
-        {
-            // the reference traps when the storage size overflows (PNG.Image.swift:84); refuse such a file here
-            const uint64_t bpp = (uint64_t)((depth * rule.channels + 7) >> 3);
-            uint64_t prod;
-            if (d.width > 0x7fffffffu || d.height > 0x7fffffffu ||
-                __builtin_mul_overflow((uint64_t)d.width * d.height, bpp ? bpp : 1, &prod) || prod > (1ull << 46))
-                return stop(PNGB200_ERR_PARSE_HEADER_SIZE, d.width, d.height, false);
-        }
-        d.depth = (uint8_t)depth, d.color = (uint8_t)color, d.interlaced = h[12];
-        d.format.color = d.color, d.format.depth = d.depth, d.format.bgr = d.standard;
-        d.storage_size = (uint64_t)d.width * d.height * (uint64_t)((depth * rule.channels + 7) >> 3);
-    }
-    bool     have_palette = false, have_background = false, have_transparency = false;
-    uint32_t npal = 0, nalpha = 0;
-    uint8_t  alpha[256];
-    for (;;) {  // up to the first IDAT
-        if (!lex()) return;
-        const ChunkRec& c = w.chunks.back();
-        const uint8_t*  body = f + c.off + 8;
-        if (c.type == CK_IHDR) return stop(PNGB200_ERR_DECODE_DUPLICATE_CHUNK, CK_IHDR, 0, false);
-        if (c.type == CK_PLTE) {
-            if (have_palette) return stop(PNGB200_ERR_DECODE_DUPLICATE_CHUNK, CK_PLTE, 0, false);
-            if (have_background) return stop(PNGB200_ERR_DECODE_UNEXPECTED_CHUNK, CK_PLTE, CK_bKGD, false);
-            if (have_transparency) return stop(PNGB200_ERR_DECODE_UNEXPECTED_CHUNK, CK_PLTE, CK_tRNS, false);
-            if (d.color == 0 || d.color == 4) return stop(PNGB200_ERR_PARSE_UNEXPECTED_PALETTE, 0, 0, false);
-            if (c.len % 3) return stop(PNGB200_ERR_PARSE_PALETTE_CHUNK_LENGTH, c.len, 0, false);
-            const uint32_t max = 1u << std::min<int>(d.depth, 8);
-            if (c.len / 3 < 1 || c.len / 3 > max) return stop(PNGB200_ERR_PARSE_PALETTE_COUNT, c.len / 3, max, false);
-            have_palette = true, npal = c.len / 3;
-            if (d.color == 3)
-                for (uint32_t i = 0; i < npal; ++i) {
-                    memcpy(d.palette_rgba + 4 * i, body + 3 * i, 3);
-                    d.palette_rgba[4 * i + 3] = 255;
-                }
-        } else if (c.type == CK_tRNS) {
-            if (have_transparency) return stop(PNGB200_ERR_DECODE_DUPLICATE_CHUNK, CK_tRNS, 0, false);
-            const uint32_t max = 0xffffu >> (16 - d.depth);
-            if (d.color == 0) {
-                if (c.len != 2) return stop(PNGB200_ERR_PARSE_TRANSPARENCY_CHUNK_LENGTH, c.len, 2, false);
-                if (load_be16(body) > max) return stop(PNGB200_ERR_PARSE_TRANSPARENCY_SAMPLE, load_be16(body), max, false);
-                d.format.has_key = 1, d.format.key[0] = (uint16_t)load_be16(body);
-            } else if (d.color == 2) {
-                if (c.len != 6) return stop(PNGB200_ERR_PARSE_TRANSPARENCY_CHUNK_LENGTH, c.len, 6, false);
-                const uint32_t r = load_be16(body), g = load_be16(body + 2), b = load_be16(body + 4);
-                if (std::max({r, g, b}) > max) return stop(PNGB200_ERR_PARSE_TRANSPARENCY_SAMPLE, std::max({r, g, b}), max, false);
-                d.format.has_key = 1;  // Format.recognize keeps a bgr8 key in (b, g, r) order (PNG.Format.swift:228-240)
-                d.format.key[0] = (uint16_t)(d.standard ? b : r), d.format.key[1] = (uint16_t)g, d.format.key[2] = (uint16_t)(d.standard ? r : b);
-            } else if (d.color == 3) {
-                if (!have_palette) return stop(PNGB200_ERR_DECODE_REQUIRED_CHUNK, CK_PLTE, CK_tRNS, false);
-                if (c.len > npal) return stop(PNGB200_ERR_PARSE_TRANSPARENCY_COUNT, c.len, npal, false);
-                memcpy(alpha, body, c.len), nalpha = c.len;
-            } else
-                return stop(PNGB200_ERR_PARSE_UNEXPECTED_TRANSPARENCY, 0, 0, false);
-            have_transparency = true;
-        } else if (c.type == CK_bKGD) {
-            if (have_background) return stop(PNGB200_ERR_DECODE_DUPLICATE_CHUNK, CK_bKGD, 0, false);
-            if (d.color == 3 && !have_palette) return stop(PNGB200_ERR_DECODE_REQUIRED_CHUNK, CK_PLTE, CK_bKGD, false);
-            have_background = true;
-        } else if (c.type == CK_cHRM || c.type == CK_gAMA || c.type == CK_sRGB || c.type == CK_iCCP || c.type == CK_sBIT) {
-            if (have_palette) return stop(PNGB200_ERR_DECODE_UNEXPECTED_CHUNK, c.type, CK_PLTE, false);
-        } else if (c.type == CK_hIST) {
-            if (!have_palette) return stop(PNGB200_ERR_DECODE_REQUIRED_CHUNK, CK_PLTE, CK_hIST, false);
-        } else if (c.type == CK_IDAT) {
-            if (d.color == 3 && !have_palette) return stop(PNGB200_ERR_DECODE_REQUIRED_CHUNK, CK_PLTE, CK_IDAT, false);
-            for (uint32_t i = 0; i < nalpha; ++i) d.palette_rgba[4 * i + 3] = alpha[i];
-            d.format.palette_count = d.color == 3 ? (uint16_t)npal : 0;
-            break;
-        } else if (c.type == CK_IEND) {
-            return stop(PNGB200_ERR_DECODE_REQUIRED_CHUNK, CK_IDAT, CK_IEND, false);
+        Tables t(ctx->h_genjobs, ctx->d_file);
+        const size_t off_files = t.host(files.data(), sizeof(WalkFile) * count);
+        const size_t off_sums = t.device(sum_bytes, false);
+        if (int rc = t.upload(ctx, t.end)) return rc;
+        png_walk_kernel<<<grid, WALK_WARPS * 32, 0, ctx->stream>>>(t.dev<WalkFile>(off_files), (uint32_t)count,
+                                                                   t.dev<WalkSummary>(off_sums), nullptr, nullptr);
+        ctx->launches++;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(t.pin<WalkSummary>(off_sums), t.dev<WalkSummary>(off_sums), sum_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        for (size_t i = 0; i < count; ++i) {
+            const WalkSummary& s = t.pin<WalkSummary>(off_sums)[i];
+            take_walk(s.head, s.palette_rgba, d[i], walks[i]);
+            base[i + 1] = base[i] + s.head.chunks;
         }
     }
-    w.first_idat = w.chunks.size() - 1;
-    while (w.chunks.back().type == CK_IDAT) {
-        d.idat_bytes += w.chunks.back().len, d.idat_chunks++;
-        w.idat_end = w.chunks.size();
-        if (!lex()) return;
-    }
-    for (;;) {  // Context.push(ancillary:) until IEND
-        const uint32_t t = w.chunks.back().type;
-        if (t == CK_IEND) return;
-        switch (t) {
-        case CK_CgBI: case CK_IHDR: case CK_PLTE: case CK_bKGD: case CK_tRNS: case CK_IDAT: case CK_hIST: case CK_cHRM:
-        case CK_gAMA: case CK_sRGB: case CK_iCCP: case CK_sBIT: case CK_pHYs: case CK_sPLT:
-            return stop(PNGB200_ERR_DECODE_UNEXPECTED_CHUNK, t, CK_IDAT, false);
-        default: break;
-        }
-        if (!lex()) return;
-    }
+    if (!records || base[count] == 0) return PNGB200_OK;
+    Tables t(ctx->h_genjobs, ctx->d_file);
+    const size_t off_files = t.host(files.data(), sizeof(WalkFile) * count);
+    const size_t off_base = t.host(base.data(), sizeof(uint64_t) * (count + 1));
+    const size_t off_sums = t.device(sum_bytes, false);
+    const size_t off_recs = t.device(sizeof(ChunkRec) * base[count], false);
+    if (int rc = t.upload(ctx, t.end)) return rc;
+    png_walk_kernel<<<grid, WALK_WARPS * 32, 0, ctx->stream>>>(t.dev<WalkFile>(off_files), (uint32_t)count, t.dev<WalkSummary>(off_sums),
+                                                               t.dev<ChunkRec>(off_recs), t.dev<uint64_t>(off_base));
+    ctx->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(t.pin<ChunkRec>(off_recs), t.dev<ChunkRec>(off_recs), sizeof(ChunkRec) * base[count], cudaMemcpyDeviceToHost,
+                       ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    for (size_t i = 0; i < count; ++i)
+        walks[i].chunks.assign(t.pin<ChunkRec>(off_recs) + base[i], t.pin<ChunkRec>(off_recs) + base[i + 1]);
+    return PNGB200_OK;
 }
 
 // CRC-32 of `regions` (device pointers) in three enqueue steps, so that a caller can put the small
@@ -331,11 +232,15 @@ int run_segment_copy(pngb200_ctx* ctx, const std::vector<CopySegment>& segs)
 // between the two); the rare file whose CRC failure changes what the decoder may see -- a bad chunk
 // before the end of its IDAT run -- is put through the exact order once more (`optimistic` = false:
 // CRCs first, then the decode of just the IDAT chunks lexed before the failure).
-int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int memspace, bool optimistic = true)
+// `device_files`: every d[i].file is device memory.  The walk then runs on the device, CRC regions point into the
+// files themselves and the IDAT run is gathered device to device; nothing else changes.
+int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int memspace, bool device_files, bool optimistic = true)
 {
     DeviceGuard guard(ctx->device);
     const bool host_pixels = memspace == PNGB200_MEM_HOST;
     std::vector<FileWalk> walks(count);
+    if (device_files)
+        if (int rc = walk_device_files(ctx, d, count, walks, true)) return rc;
     // Device image of a file: [bytes in front of the first IDAT | bytes behind the IDAT run] in the file
     // arena, and the bodies of the IDAT run back to back in the payload arena.  The H2D copy itself
     // does the concatenation: a run of equal-sized IDAT chunks (what every encoder writes, the reference
@@ -343,30 +248,33 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
     std::vector<size_t> f_off(count), g_off(count), pre_len(count), post_at(count), post_len(count);
     Slots files{16}, payloads{16};
     for (size_t i = 0; i < count; ++i) {
-        if (!d[i].file && d[i].file_len) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "file %zu: null pointer", i);
         FileWalk& w = walks[i];
-        walk_file(d[i], w);
-        d[i].chunks = (uint32_t)w.chunks.size();
+        if (!device_files) {
+            if (!d[i].file && d[i].file_len) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "file %zu: null pointer", i);
+            walk_file(d[i], w);
+        }
         d[i].status = PNGB200_OK, d[i].err_a = d[i].err_b = 0;
         d[i].checksum = d[i].blocks = 0, d[i].produced = 0;
         if (w.first_idat != (size_t)-1 && (!d[i].pixels || d[i].pixels_cap < d[i].storage_size))
             return set_error(ctx, PNGB200_ERR_OUTPUT_CAPACITY, "file %zu: pixels_cap %zu < %llu", i, d[i].pixels_cap,
                              (unsigned long long)d[i].storage_size);
         const size_t lexed = w.chunks.empty() ? 0 : (size_t)(w.chunks.back().off + 12 + w.chunks.back().len);
-        if (w.first_idat == (size_t)-1) {
+        if (device_files) {
+            pre_len[i] = post_at[i] = post_len[i] = 0;  // nothing staged: the CRC pass reads the file where it is
+        } else if (w.first_idat == (size_t)-1) {
             pre_len[i] = lexed, post_at[i] = lexed, post_len[i] = 0;
         } else {
             pre_len[i] = (size_t)w.chunks[w.first_idat].off;
             post_at[i] = w.idat_end < w.chunks.size() ? (size_t)w.chunks[w.idat_end].off : lexed;
             post_len[i] = lexed - post_at[i];
         }
-        f_off[i] = files.add(pre_len[i] + post_len[i]);
+        if (!device_files) f_off[i] = files.add(pre_len[i] + post_len[i]);
         g_off[i] = payloads.add(d[i].idat_bytes);
     }
-    CU(ctx->d_file.reserve(std::max<size_t>(files.total, 256)));
+    if (!device_files) CU(ctx->d_file.reserve(std::max<size_t>(files.total, 256)));
     CU(ctx->d_in.reserve(std::max<size_t>(payloads.total, 256)));
-    // every lexed chunk's CRC region (type + body): in the file arena, or -- IDAT run -- the body in the
-    // payload arena with the type folded in as a prefix
+    // every lexed chunk's CRC region (type + body): in the device file; else in the file arena, or -- IDAT run -- the
+    // body in the payload arena with the type folded in as a prefix
     std::vector<CrcRegion> regions;
     std::vector<size_t>    region_base(count + 1);
     for (size_t i = 0; i < count; ++i) {
@@ -376,7 +284,9 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
         uint8_t*        body = ctx->d_in.as<uint8_t>() + g_off[i];
         for (size_t k = 0; k < w.chunks.size(); ++k) {
             const ChunkRec& c = w.chunks[k];
-            if (w.first_idat != (size_t)-1 && k >= w.first_idat && k < w.idat_end) {
+            if (device_files) {
+                regions.push_back({d[i].file + c.off + 4, (uint64_t)c.len + 4, 0, 0});
+            } else if (w.first_idat != (size_t)-1 && k >= w.first_idat && k < w.idat_end) {
                 regions.push_back({body, (uint64_t)c.len, CK_IDAT, 1});
                 body += c.len;
             } else {
@@ -386,13 +296,13 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
         }
     }
     region_base[count] = regions.size();
+    const cudaMemcpyKind kind = device_files ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     auto upload_files = [&]() -> int {
         for (size_t i = 0; i < count; ++i) {
             const FileWalk& w = walks[i];
             uint8_t* const  meta = ctx->d_file.as<uint8_t>() + f_off[i];
-            if (pre_len[i]) CU(cudaMemcpyAsync(meta, d[i].file, pre_len[i], cudaMemcpyHostToDevice, ctx->stream));
-            if (post_len[i])
-                CU(cudaMemcpyAsync(meta + pre_len[i], d[i].file + post_at[i], post_len[i], cudaMemcpyHostToDevice, ctx->stream));
+            if (pre_len[i]) CU(cudaMemcpyAsync(meta, d[i].file, pre_len[i], kind, ctx->stream));
+            if (post_len[i]) CU(cudaMemcpyAsync(meta + pre_len[i], d[i].file + post_at[i], post_len[i], kind, ctx->stream));
             if (w.first_idat == (size_t)-1) continue;
             uint8_t* body = ctx->d_in.as<uint8_t>() + g_off[i];
             for (size_t k = w.first_idat; k < w.idat_end;) {
@@ -402,9 +312,9 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
                 const uint8_t* src = d[i].file + w.chunks[k].off + 8;
                 if (len == 0) {
                 } else if (run == 1) {
-                    CU(cudaMemcpyAsync(body, src, len, cudaMemcpyHostToDevice, ctx->stream));
+                    CU(cudaMemcpyAsync(body, src, len, kind, ctx->stream));
                 } else {
-                    CU(cudaMemcpy2DAsync(body, len, src, (size_t)len + 12, len, run, cudaMemcpyHostToDevice, ctx->stream));
+                    CU(cudaMemcpy2DAsync(body, len, src, (size_t)len + 12, len, run, kind, ctx->stream));
                 }
                 body += (size_t)len * run;
                 k += run;
@@ -526,7 +436,7 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
     if (!redo.empty()) {
         std::vector<pngb200_png_desc> again(redo.size());
         for (size_t r = 0; r < redo.size(); ++r) again[r] = d[redo[r]];
-        rc = png_decode_some(ctx, again.data(), again.size(), memspace, false);
+        rc = png_decode_some(ctx, again.data(), again.size(), memspace, device_files, false);
         if (rc != PNGB200_OK) return rc;
         for (size_t r = 0; r < redo.size(); ++r) {
             d[redo[r]] = again[r];
@@ -540,28 +450,53 @@ int png_decode_some(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int mem
 
 extern "C" {
 
-int pngb200_png_inspect_batch(pngb200_png_desc* d, size_t count)
+int pngb200_png_inspect_files(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int file_memspace)
 {
     if (!d && count) return PNGB200_ERR_BAD_ARGUMENT;
-    for (size_t i = 0; i < count; ++i) {
-        if (!d[i].file && d[i].file_len) return PNGB200_ERR_BAD_ARGUMENT;
-        FileWalk w;
-        walk_file(d[i], w);
-        d[i].chunks = (uint32_t)w.chunks.size();
+    std::vector<FileWalk> walks(count);
+    auto report = [&](size_t i) {
+        const FileWalk& w = walks[i];
         d[i].status = w.status, d[i].err_a = w.a, d[i].err_b = w.b;
         d[i].checksum = d[i].blocks = 0, d[i].produced = 0;
+    };
+    if (file_memspace == PNGB200_MEM_HOST) {
+        for (size_t i = 0; i < count; ++i) {
+            if (!d[i].file && d[i].file_len) return PNGB200_ERR_BAD_ARGUMENT;
+            walk_file(d[i], walks[i]);
+            report(i);
+        }
+        return PNGB200_OK;
     }
+    if (file_memspace != PNGB200_MEM_DEVICE) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "file_memspace %d", file_memspace);
+    if (!ctx) return PNGB200_ERR_BAD_ARGUMENT;
+    if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a decode batch is pending");
+    DeviceGuard guard(ctx->device);
+    if (int rc = walk_device_files(ctx, d, count, walks, false)) return rc;
+    for (size_t i = 0; i < count; ++i) report(i);
     return PNGB200_OK;
+}
+
+int pngb200_png_inspect_batch(pngb200_png_desc* d, size_t count)
+{
+    return pngb200_png_inspect_files(nullptr, d, count, PNGB200_MEM_HOST);
+}
+
+int pngb200_png_decode_files(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int file_memspace, int memspace)
+{
+    if (!ctx || (!d && count)) return PNGB200_ERR_BAD_ARGUMENT;
+    if (file_memspace != PNGB200_MEM_HOST && file_memspace != PNGB200_MEM_DEVICE)
+        return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "file_memspace %d", file_memspace);
+    if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a decode batch is pending");
+    if (count == 0) return PNGB200_OK;
+    if (file_memspace == PNGB200_MEM_DEVICE) return png_decode_some(ctx, d, count, memspace, true);  // no H2D copy to overlap
+    return run_over_lanes(ctx, count, memspace,
+                          [&](size_t i) { return d[i].file_len + (size_t)0; },
+                          [&](pngb200_ctx* lane, size_t lo, size_t n) { return png_decode_some(lane, d + lo, n, memspace, false); });
 }
 
 int pngb200_png_decode_batch(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count, int memspace)
 {
-    if (!ctx || (!d && count)) return PNGB200_ERR_BAD_ARGUMENT;
-    if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a decode batch is pending");
-    if (count == 0) return PNGB200_OK;
-    return run_over_lanes(ctx, count, memspace,
-                          [&](size_t i) { return d[i].file_len + (size_t)0; },
-                          [&](pngb200_ctx* lane, size_t lo, size_t n) { return png_decode_some(lane, d + lo, n, memspace); });
+    return pngb200_png_decode_files(ctx, d, count, PNGB200_MEM_HOST, memspace);
 }
 
 size_t pngb200_png_encode_bound(uint32_t width, uint32_t height, const pngb200_pixel_format* f, int interlaced, uint32_t idat_chunk)
@@ -573,9 +508,12 @@ size_t pngb200_png_encode_bound(uint32_t width, uint32_t height, const pngb200_p
     return 8 + 16 + 25 + (12 + 768) + (12 + 256) + z + 12 * (z / chunk + 2) + 12 + 64;
 }
 
-int pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_t count, int memspace)
+int pngb200_png_encode_files(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_t count, int memspace, int file_memspace)
 {
     if (!ctx || (!d && count)) return PNGB200_ERR_BAD_ARGUMENT;
+    if (file_memspace != PNGB200_MEM_HOST && file_memspace != PNGB200_MEM_DEVICE)
+        return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "file_memspace %d", file_memspace);
+    const bool host_files = file_memspace == PNGB200_MEM_HOST;
     if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a decode batch is pending");
     if (count == 0) return PNGB200_OK;
     DeviceGuard guard(ctx->device);
@@ -670,7 +608,8 @@ int pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_
     }
     int rc = pngb200_encode_batch(ctx, enc.data(), count, PNGB200_MEM_DEVICE);
     if (rc != PNGB200_OK) return rc;
-    // stage 2: frame the payload into IDAT chunks inside a device image of the file, CRC them there
+    // stage 2: frame the payload into IDAT chunks inside a device image of the file (device files: the file itself),
+    // CRC them there
     std::vector<size_t> file_off(count), file_len(count);
     Slots files{16};
     std::vector<FrameItem>   frames;
@@ -682,12 +621,12 @@ int pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_
         const size_t chunk = d[i].idat_chunk ? d[i].idat_chunk : 65544;
         const size_t z = enc[i].produced, nchunks = (z + chunk - 1) / chunk;
         file_len[i] = head_len[i] + z + 12 * nchunks + 12;
-        file_off[i] = files.add(file_len[i]);
+        if (host_files) file_off[i] = files.add(file_len[i]);
     }
-    CU(ctx->d_file.reserve(std::max<size_t>(files.total, 256)));
+    if (host_files) CU(ctx->d_file.reserve(std::max<size_t>(files.total, 256)));
     for (size_t i = 0; i < count; ++i) {
         if (enc[i].status != PNGB200_OK) continue;
-        uint8_t* base = ctx->d_file.as<uint8_t>() + file_off[i];
+        uint8_t* base = host_files ? ctx->d_file.as<uint8_t>() + file_off[i] : d[i].file;
         CU(cudaMemcpyAsync(base, heads[i].data(), head_len[i], cudaMemcpyHostToDevice, ctx->stream));
         const size_t chunk = d[i].idat_chunk ? d[i].idat_chunk : 65544;
         // Encoder.pull hands out DeflatorOut's queued buffers (2 x capacity bytes each), then the rest
@@ -724,11 +663,17 @@ int pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_
     }
     for (size_t i = 0; i < count; ++i) {
         if (enc[i].status != PNGB200_OK) continue;
-        CU(cudaMemcpyAsync(d[i].file, ctx->d_file.as<uint8_t>() + file_off[i], file_len[i], cudaMemcpyDeviceToHost, ctx->stream));
+        if (host_files)
+            CU(cudaMemcpyAsync(d[i].file, ctx->d_file.as<uint8_t>() + file_off[i], file_len[i], cudaMemcpyDeviceToHost, ctx->stream));
         d[i].produced = file_len[i];
     }
     CU(cudaStreamSynchronize(ctx->stream));
     return PNGB200_OK;
+}
+
+int pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_t count, int memspace)
+{
+    return pngb200_png_encode_files(ctx, d, count, memspace, PNGB200_MEM_HOST);
 }
 
 }  // extern "C"

@@ -26,6 +26,7 @@
 #include "block_search.cuh"
 #include "inflate_segments.cuh"
 #include "inflate_serial.cuh"
+#include "png_walk.cuh"
 #include "unfilter.cuh"
 
 using namespace pngb200;
@@ -214,22 +215,6 @@ struct Tables {
     template <typename T> T* dev(size_t off) const { return (T*)((char*)d.p + off); }
     template <typename T> T* pin(size_t off) const { return (T*)((char*)h.p + off); }
 };
-
-// PNG.Format.Pixel.recognize(code:): whether (color, depth, bgr) is a pixel format (bgr, the iOS byte order: 8-bit
-// RGB and RGBA only), and the channels of colour type `color` (4 for a type that does not exist)
-struct PixelRule { bool valid; int channels; };
-PixelRule pixel_rule(int color, int depth, bool bgr)
-{
-    bool ok;
-    switch (color) {
-    case 0: ok = depth == 1 || depth == 2 || depth == 4 || depth == 8 || depth == 16; break;
-    case 3: ok = depth == 1 || depth == 2 || depth == 4 || depth == 8; break;
-    case 2: case 4: case 6: ok = depth == 8 || depth == 16; break;
-    default: ok = false;
-    }
-    if (bgr && (depth != 8 || (color != 2 && color != 6))) ok = false;
-    return {ok, color == 0 || color == 3 ? 1 : color == 2 ? 3 : color == 4 ? 2 : 4};
-}
 
 // the CRC-32 byte table and shift operators (crc32.cuh), uploaded once per context
 int ensure_crc_tables(pngb200_ctx* ctx)
