@@ -150,8 +150,16 @@ int          pngb200_ctx_last_inflate_engine(pngb200_ctx* ctx);
 /* scanlines per filter type of the last decode / unfilter batch that went through the wavefront kernel
  * (non-interlaced, >= 8 bits per sample): out[0..4] = None, Sub, Up, Average, Paeth, out[5] = rows with an
  * invalid filter byte (left unchanged, as the reference does).  The device-side form of the reference's
- * -DDUMP_FILTERED_SCANLINES output (Sources/PNG/Decoding/PNG.Decoder.swift:96-98,128). */
+ * -DDUMP_FILTERED_SCANLINES output (Sources/PNG/Decoding/PNG.Decoder.swift:96-98,128).  Rows of Adam7 and
+ * 1/2/4-bit images are not counted, whichever kernel reconstructs them. */
 int          pngb200_ctx_filter_histogram(pngb200_ctx* ctx, uint64_t out[6]);
+/* images of the last decode / unfilter batch by the path that reconstructed their scanlines: out[0] the wavefront
+ * kernel (non-interlaced, >= 8 bits per sample), out[1] the pass path (Adam7 or 1/2/4-bit images whose filtered
+ * stream is longer than 64 KiB: every pass on the wavefront, then one interleave kernel), out[2] the one-CTA-per-image
+ * generic kernel (the other Adam7 and 1/2/4-bit images).  Results are identical whichever path runs.  A batch starts
+ * with pngb200_decode_batch, pngb200_unfilter_batch and the PNG file decode calls; a direct
+ * pngb200_decode_batch_enqueue adds its images to the batch in progress. */
+int          pngb200_ctx_unfilter_stats(pngb200_ctx* ctx, uint64_t out[3]);
 /* inflate_mode: 0 automatic; 1 one warp per stream; 2 a whole CTA per stream, never cut; 3 / 4 force the
  * ring-window / the round-1 intra-stream kernel; 5 as 0; 6 force the cell kernel (inflate_cells.cuh) */
 

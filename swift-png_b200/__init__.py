@@ -247,6 +247,9 @@ def lib():
     L.pngb200_ctx_filter_histogram.restype = C.c_int
     L.pngb200_ctx_segment_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     L.pngb200_ctx_segment_stats.restype = C.c_int
+    if os.environ.get("PNGB200_LIB") is None or hasattr(L, "pngb200_ctx_unfilter_stats"):   # (older builds lack it)
+        L.pngb200_ctx_unfilter_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.pngb200_ctx_unfilter_stats.restype = C.c_int
     if os.environ.get("PNGB200_LIB") is None or hasattr(L, "pngb200_ctx_split_stats"):   # (older tuning builds lack it)
         L.pngb200_ctx_split_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
         L.pngb200_ctx_split_stats.restype = C.c_int
@@ -372,6 +375,13 @@ class Context:
         out = (C.c_uint64 * 3)()
         self.check(self._lib.pngb200_ctx_segment_stats(self.handle, out))
         return dict(streams=out[0], segments=out[1], fallbacks=out[2])
+
+    def unfilter_stats(self):
+        """images of the last decode / unfilter batch by unfilter path: the wavefront kernel (non-interlaced, >= 8 bits),
+        the pass path (Adam7 and 1/2/4-bit images past 64 KiB of filtered stream) and the one-CTA generic kernel"""
+        out = (C.c_uint64 * 3)()
+        self.check(self._lib.pngb200_ctx_unfilter_stats(self.handle, out))
+        return dict(wavefront=out[0], passes=out[1], generic=out[2])
 
     def split_stats(self):
         """bytes and SM cycles of the heads and tails of the streams the last batch cut in two, the tails that left

@@ -488,7 +488,10 @@ int pngb200_png_decode_files(pngb200_ctx* ctx, pngb200_png_desc* d, size_t count
         return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "file_memspace %d", file_memspace);
     if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a decode batch is pending");
     if (count == 0) return PNGB200_OK;
-    if (file_memspace == PNGB200_MEM_DEVICE) return png_decode_some(ctx, d, count, memspace, true);  // no H2D copy to overlap
+    if (file_memspace == PNGB200_MEM_DEVICE) {   // no H2D copy to overlap
+        start_unfilter_stats(ctx);
+        return png_decode_some(ctx, d, count, memspace, true);
+    }
     return run_over_lanes(ctx, count, memspace,
                           [&](size_t i) { return d[i].file_len + (size_t)0; },
                           [&](pngb200_ctx* lane, size_t lo, size_t n) { return png_decode_some(lane, d + lo, n, memspace, false); });

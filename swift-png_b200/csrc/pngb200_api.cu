@@ -120,6 +120,7 @@ struct pngb200_ctx {
     uint64_t scratch_stride = 0;       // layout of d_scratch the last inflate launch used
     size_t parallel_threshold = 8192;  // streams at least this long use the block-parallel kernel
     unsigned long long* d_hist = nullptr;   // filter-type histogram of the last wavefront-unfilter launch (in d_imgjobs)
+    uint64_t unfilter_images[3] = {};  // images of the batch by unfilter path: wavefront, pass path, generic kernel
     size_t peer_streams = 0;           // lanes: streams of the whole host batch (its chunks run side by side on this GPU)
     bool   split = true;               // cut big streams into a head and a tail when that evens out the CTA slots (PNGB200_SPLIT=0: off)
     size_t plan_slots = 0;             // CTA slots the segment and split planners assume, 0 = the ring kernel's (PNGB200_PLAN_SLOTS:
@@ -744,6 +745,7 @@ struct Geometry {
     uint32_t pitch;     // non-interlaced pitch
     uint8_t  bpp;
     bool     fast;      // eligible for the wavefront kernel
+    bool     passes;    // Adam7 or 1/2/4-bit samples in a PNG layout: eligible for the pass path (see run_unfilter)
 };
 
 bool geometry(uint32_t w, uint32_t h, int volume, int depth, int interlaced, Geometry* g)
@@ -765,7 +767,19 @@ bool geometry(uint32_t w, uint32_t h, int volume, int depth, int interlaced, Geo
     g->bpp      = (uint8_t)((volume + 7) >> 3);
     g->fast     = !interlaced && depth >= 8 &&
               (g->bpp == 1 || g->bpp == 2 || g->bpp == 3 || g->bpp == 4 || g->bpp == 6 || g->bpp == 8);
+    // whole bytes per pixel with the wavefront's filter distances, or one 1/2/4-bit sample per pixel
+    const bool layout = depth >= 8 ? volume % 8 == 0 && (g->bpp <= 4 || g->bpp == 6 || g->bpp == 8)
+                                   : volume == depth && (depth == 1 || depth == 2 || depth == 4);
+    g->passes   = !g->fast && layout;
     return true;
+}
+
+// a decode or unfilter batch starts: its images are counted from zero on the context and on its lanes
+void start_unfilter_stats(pngb200_ctx* ctx)
+{
+    for (pngb200_ctx* lane : ctx->lanes)
+        for (uint64_t& n : lane->unfilter_images) n = 0;
+    for (uint64_t& n : ctx->unfilter_images) n = 0;
 }
 
 // unfilter stage over device-resident filtered streams
@@ -780,16 +794,93 @@ struct UnfilterItem {
     Geometry            g;
 };
 
+// Images of the pass path (Adam7 or 1/2/4-bit) whose filtered stream is at most this long go to
+// unfilter_generic_kernel instead: below it, planning up to seven jobs an image and two launches cost more than one CTA
+// per image spends on its rows (DESIGN §4.3, the size sweep of tools/unfilter_passes_bw.py).
+constexpr uint64_t UNFILTER_GENERIC_MAX = 65536;
+
+// The wavefront's ticket order over `jobs` (ImageJob or PassJob, `height` rows each).  Tickets go out band level by band
+// level (see WaveParams): jobs sorted by band count, descending; level_start[b] = tickets in front of level b.  (Jobs of
+// more than 4096 bands -- 131072 rows -- keep the job-major order and leave level_start empty.)  band_base[i] = the
+// first band of job i.  Returns the number of bands.
+template <typename Job>
+uint64_t plan_bands(std::vector<Job>& jobs, std::vector<uint32_t>& band_base, std::vector<uint32_t>& level_start)
+{
+    auto nb = [&](const Job& j) { return (j.height + 31) / 32; };
+    level_start.clear();
+    std::vector<uint32_t> idx(jobs.size());
+    for (size_t i = 0; i < idx.size(); ++i) idx[i] = (uint32_t)i;
+    std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return nb(jobs[a]) > nb(jobs[b]); });
+    const uint32_t maxb = jobs.empty() ? 0 : nb(jobs[idx[0]]);
+    if (!jobs.empty() && maxb <= 4096) {
+        std::vector<Job> sorted(jobs.size());
+        for (size_t i = 0; i < idx.size(); ++i) sorted[i] = jobs[idx[i]];
+        jobs.swap(sorted);
+        level_start.assign(maxb + 1, 0);
+        size_t alive = jobs.size();          // jobs with more than b bands: a prefix of the sorted list
+        for (uint32_t b = 0; b < maxb; ++b) {
+            while (alive && nb(jobs[alive - 1]) <= b) --alive;
+            level_start[b + 1] = level_start[b] + (uint32_t)alive;
+        }
+    }
+    band_base.assign(jobs.size() + 1, 0);
+    uint64_t bands = 0;
+    for (size_t i = 0; i < jobs.size(); ++i) {
+        band_base[i] = (uint32_t)std::min<uint64_t>(bands, UINT32_MAX);
+        bands += nb(jobs[i]);
+    }
+    band_base[jobs.size()] = (uint32_t)std::min<uint64_t>(bands, UINT32_MAX);
+    return bands;
+}
+
 int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
 {
     ctx->d_hist = nullptr;
 
     std::vector<ImageJob>   fast;
     std::vector<GenericJob> slow;
+    std::vector<PassJob>    pass;
+    std::vector<InterleaveJob> inter;
     std::vector<uint32_t>   band_base;
-    uint64_t                bands = 0;
+    uint64_t                inter_blocks = 0;
     for (const UnfilterItem& it : items) {
-        if (it.g.fast) {
+        if (it.g.passes && it.g.filtered > UNFILTER_GENERIC_MAX) {
+            // one job per non-empty Adam7 pass, or one for a non-interlaced 1/2/4-bit image, at its offset in the stream
+            uint64_t off = 0;
+            for (int z = 0; z < (it.interlaced ? 7 : 1); ++z) {
+                uint64_t sw = it.w, sh = it.h;
+                if (it.interlaced) {
+                    sw = ((uint64_t)it.w + (1u << ADAM7[z][2]) - ADAM7[z][0] - 1) >> ADAM7[z][2];
+                    sh = ((uint64_t)it.h + (1u << ADAM7[z][3]) - ADAM7[z][1] - 1) >> ADAM7[z][3];
+                    if (sw == 0 || sh == 0) continue;
+                }
+                PassJob j;
+                j.pitch = (uint32_t)((sw * it.volume + 7) >> 3);
+                j.filtered = it.filtered_mut + off;
+                j.inflated = it.inflated;
+                j.filtered_len = it.filtered_len;
+                j.offset = off;
+                j.height = (uint32_t)sh;
+                j.bpp = it.g.bpp;
+                pass.push_back(j);
+                off += sh * ((uint64_t)j.pitch + 1);
+            }
+            InterleaveJob j;
+            j.filtered = it.filtered_mut;
+            j.pixels = it.pixels;
+            j.inflated = it.inflated;
+            j.filtered_len = it.filtered_len;
+            j.block_base = inter_blocks;
+            j.width = it.w;
+            j.height = it.h;
+            j.volume = it.volume;
+            j.depth = it.depth;
+            j.interlaced = it.interlaced;
+            j.bpp = it.g.bpp;
+            inter.push_back(j);
+            const uint64_t chunks = (15 + it.g.storage + 15) / 16;   // any misalignment of the pixels
+            inter_blocks += (chunks + INTERLEAVE_THREADS - 1) / INTERLEAVE_THREADS;
+        } else if (it.g.fast) {
             ImageJob j;
             j.filtered = it.filtered;
             j.pixels = it.pixels;
@@ -803,8 +894,6 @@ int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
             j.interlaced = 0;
             j.bpp = it.g.bpp;
             fast.push_back(j);
-            band_base.push_back((uint32_t)bands);
-            bands += (it.h + 31) / 32;
         } else {
             GenericJob j;
             j.filtered = it.filtered_mut;
@@ -820,35 +909,15 @@ int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
             slow.push_back(j);
         }
     }
-    band_base.push_back((uint32_t)bands);
-    if (bands >= (1ull << 31)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
+    // the fast and the pass path hand out their bands level by level
+    std::vector<uint32_t> level_start, pass_base, pass_levels;
+    const uint64_t bands = plan_bands(fast, band_base, level_start);
+    const uint64_t pass_bands = plan_bands(pass, pass_base, pass_levels);
+    if (bands >= (1ull << 31) || pass_bands >= (1ull << 31)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "batch too large");
+    ctx->unfilter_images[0] += fast.size();
+    ctx->unfilter_images[1] += inter.size();
+    ctx->unfilter_images[2] += slow.size();
     if (!fast.empty()) {
-        // Tickets go out band level by band level (see WaveParams): jobs sorted by band count, descending; level_start[b] =
-        // tickets in front of level b.  (Images of more than 4096 bands -- 131072 rows -- keep the image-major order.)
-        std::vector<uint32_t> level_start;
-        {
-            std::vector<uint32_t> idx(fast.size());
-            for (size_t i = 0; i < idx.size(); ++i) idx[i] = (uint32_t)i;
-            auto nb = [&](uint32_t i) { return (fast[i].height + 31) / 32; };
-            std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return nb(a) > nb(b); });
-            const uint32_t maxb = nb(idx[0]);
-            if (maxb <= 4096) {
-                std::vector<ImageJob> sorted(fast.size());
-                for (size_t i = 0; i < idx.size(); ++i) sorted[i] = fast[idx[i]];
-                fast.swap(sorted);
-                uint64_t at = 0;
-                for (size_t i = 0; i < fast.size(); ++i) {
-                    band_base[i] = (uint32_t)at;
-                    at += (fast[i].height + 31) / 32;
-                }
-                level_start.assign(maxb + 1, 0);
-                size_t alive = fast.size();          // images with more than b bands: a prefix of the sorted list
-                for (uint32_t b = 0; b < maxb; ++b) {
-                    while (alive && (fast[alive - 1].height + 31) / 32 <= b) --alive;
-                    level_start[b + 1] = level_start[b] + (uint32_t)alive;
-                }
-            }
-        }
         Tables t(ctx->h_imgjobs, ctx->d_imgjobs);
         const size_t off_jobs = t.host(fast.data(), sizeof(ImageJob) * fast.size());
         const size_t off_bb = t.host(band_base.data(), sizeof(uint32_t) * band_base.size());
@@ -875,11 +944,40 @@ int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
         ctx->launches++;
         CU(cudaGetLastError());
     }
+    if (pass.empty() && slow.empty()) return PNGB200_OK;
+    // the pass path and the generic kernel share one table upload
+    Tables t(ctx->h_genjobs, ctx->d_genjobs);
+    const size_t off_gen = t.host(slow.data(), sizeof(GenericJob) * slow.size());
+    const size_t off_pass = t.host(pass.data(), sizeof(PassJob) * pass.size());
+    const size_t off_pb = t.host(pass_base.data(), sizeof(uint32_t) * pass_base.size());
+    const size_t off_pl = t.host(pass_levels.data(), sizeof(uint32_t) * pass_levels.size());
+    const size_t off_inter = t.host(inter.data(), sizeof(InterleaveJob) * inter.size());
+    const size_t off_pr = t.device(sizeof(uint32_t) * (pass_bands + 1), true);   // per-band progress, then the ticket
+    if (int rc = t.upload(ctx)) return rc;
+    if (!pass.empty()) {
+        WaveParams p;
+        p.jobs = t.dev<PassJob>(off_pass);
+        p.band_base = t.dev<uint32_t>(off_pb);
+        p.progress = t.dev<uint32_t>(off_pr);
+        p.ticket = p.progress + pass_bands;
+        p.hist = nullptr;
+        p.njobs = (uint32_t)pass.size();
+        p.total_bands = (uint32_t)pass_bands;
+        p.level_start = t.dev<uint32_t>(off_pl);
+        p.levels = pass_levels.empty() ? 0u : (uint32_t)pass_levels.size() - 1;
+        unsigned grid = (unsigned)std::min<uint64_t>((pass_bands + WAVE_WARPS - 1) / WAVE_WARPS,
+                                                     (uint64_t)ctx->sm_count * 8);
+        unfilter_pass_kernel<<<grid, WAVE_WARPS * 32, WAVE_SMEM, ctx->stream>>>(p);
+        ctx->launches++;
+        CU(cudaGetLastError());
+        grid = (unsigned)std::min<uint64_t>(inter_blocks, (uint64_t)ctx->sm_count * 16);
+        unfilter_interleave_kernel<<<grid, INTERLEAVE_THREADS, 0, ctx->stream>>>(t.dev<InterleaveJob>(off_inter),
+                                                                                 (uint32_t)inter.size(), inter_blocks);
+        ctx->launches++;
+        CU(cudaGetLastError());
+    }
     if (!slow.empty()) {
-        Tables t(ctx->h_genjobs, ctx->d_genjobs);
-        const size_t off_jobs = t.host(slow.data(), sizeof(GenericJob) * slow.size());
-        if (int rc = t.upload(ctx)) return rc;
-        unfilter_generic_kernel<<<(unsigned)slow.size(), 128, 0, ctx->stream>>>(t.dev<GenericJob>(off_jobs), (int)slow.size());
+        unfilter_generic_kernel<<<(unsigned)slow.size(), 128, 0, ctx->stream>>>(t.dev<GenericJob>(off_gen), (int)slow.size());
         ctx->launches++;
         CU(cudaGetLastError());
     }
@@ -899,6 +997,7 @@ int run_over_lanes(pngb200_ctx* ctx, size_t count, int memspace, BytesOf bytes_o
 {
     for (pngb200_ctx* lane : ctx->lanes) lane->d_hist = nullptr;   // counters describe the batch that starts now
     ctx->d_hist = nullptr;
+    start_unfilter_stats(ctx);
     size_t bytes = 0;
     for (size_t i = 0; i < count; ++i) bytes += bytes_of(i);
     // tunable for experiments: PNGB200_LANES, PNGB200_CHUNKS_PER_LANE (0 / unset = the rule above); read once
@@ -1007,7 +1106,8 @@ pngb200_ctx* pngb200_ctx_create(int device)
     const std::pair<const void*, size_t> opt_in[] = {
         {(const void*)deflate_kernel, sizeof(DfShared)},          {(const void*)inflate_parallel_kernel3, sizeof(ParShared)},
         {(const void*)inflate_parallel_kernel, sizeof(ParShared)}, {(const void*)inflate_wave_kernel, sizeof(WvShared)},
-        {(const void*)unfilter_wave_kernel, WAVE_SMEM},           {(const void*)inflate_cells_kernel, sizeof(ClShared)}};
+        {(const void*)unfilter_wave_kernel, WAVE_SMEM},           {(const void*)inflate_cells_kernel, sizeof(ClShared)},
+        {(const void*)unfilter_pass_kernel, WAVE_SMEM}};
     for (const auto& [kernel, bytes] : opt_in)
         if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess) {
             set_error(nullptr, PNGB200_ERR_CUDA, "cannot opt in to %zu bytes of shared memory", bytes);
@@ -1111,6 +1211,16 @@ int pngb200_ctx_filter_histogram(pngb200_ctx* ctx, uint64_t out[6])
 }
 
 int pngb200_ctx_last_inflate_engine(pngb200_ctx* ctx) { return ctx ? ctx->last_engine : -1; }
+
+int pngb200_ctx_unfilter_stats(pngb200_ctx* ctx, uint64_t out[3])
+{
+    if (!ctx || !out) return PNGB200_ERR_BAD_ARGUMENT;
+    for (int k = 0; k < 3; ++k) {
+        out[k] = ctx->unfilter_images[k];
+        for (const pngb200_ctx* lane : ctx->lanes) out[k] += lane->unfilter_images[k];
+    }
+    return PNGB200_OK;
+}
 
 int pngb200_ctx_split_stats(pngb200_ctx* ctx, uint64_t out[6])
 {
@@ -1328,6 +1438,7 @@ int pngb200_unfilter_batch(pngb200_ctx* ctx, pngb200_image_desc* im, size_t coun
     if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a decode batch is pending");
     if (count == 0) return PNGB200_OK;
     DeviceGuard guard(ctx->device);
+    start_unfilter_stats(ctx);
     const bool host = memspace == PNGB200_MEM_HOST;
     std::vector<UnfilterItem> items(count);
     std::vector<size_t>       f_off(count), o_off(count);
@@ -1338,7 +1449,7 @@ int pngb200_unfilter_batch(pngb200_ctx* ctx, pngb200_image_desc* im, size_t coun
             !im[i].idat || !im[i].pixels)
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: bad descriptor", i);
         if (im[i].pixels_cap < it.g.storage) return set_error(ctx, PNGB200_ERR_OUTPUT_CAPACITY, "image %zu: pixels_cap", i);
-        // the generic kernel reconstructs in place, so it always works on a private copy
+        // the generic kernel and the pass path reconstruct in place, so they always work on a private copy
         if (host || !it.g.fast) f_off[i] = f.add(im[i].idat_len);
         o_off[i] = o.add(it.g.storage);
     }

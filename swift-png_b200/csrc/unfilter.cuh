@@ -16,8 +16,16 @@
 //   shared-memory ring in 16-byte chunks (see WAVE_DEPTH) and writes its chunks in pairs: two
 //   back-to-back 16-byte stores that fill a whole 32-byte sector (see wave_band).
 //
-// unfilter_generic_kernel: every other format (Adam7, 1/2/4-bit samples); one CTA per image.
+// unfilter_pass_kernel (Adam7 and 1/2/4-bit images whose filtered stream is longer than UNFILTER_GENERIC_MAX):
+//   the same wavefront over PassJobs.  An Adam7 pass is an ordinary filtered image of its own width and height with
+//   the image's filter distance, and the rows of a 1/2/4-bit image are byte rows with filter distance 1, so each pass
+//   (or the whole sub-byte image) is one job.  Rows are reconstructed in place in the library's private copy of the
+//   filtered stream; unfilter_interleave_kernel then writes PNG.Image.storage from the pass rows.
+//
+// unfilter_generic_kernel: the same formats when the filtered stream is short; one CTA per image.
 #pragma once
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -109,8 +117,19 @@ __device__ __forceinline__ void store16_partial(uint8_t* p, uint4 v, int nbytes)
     }
 }
 
+// One Adam7 pass of an image, or the whole of a non-interlaced 1/2/4-bit image, for unfilter_pass_kernel.  Its rows are
+// reconstructed in place: the pixels of row y overwrite that row's filtered bytes, at stride pitch + 1, offset 1.
+struct PassJob {
+    uint8_t*            filtered;      // the pass's first filter byte in the image's private (mutable) filtered stream
+    const StreamResult* inflated;      // the image's producer result, as ImageJob; may be null
+    uint64_t            filtered_len;  // used when `inflated` is null
+    uint64_t            offset;        // bytes of the image's stream in front of the pass
+    uint32_t            height, pitch; // rows and bytes per row of the pass
+    uint32_t            bpp;           // filter distance
+};
+
 struct WaveParams {
-    const ImageJob* jobs;
+    const void*     jobs;       // ImageJob[] (unfilter_wave_kernel) or PassJob[] (unfilter_pass_kernel)
     const uint32_t* band_base;  // [njobs + 1] exclusive prefix of ceil(h/32)
     uint32_t*       progress;   // [total_bands]
     uint32_t*       ticket;
@@ -162,14 +181,39 @@ __device__ __forceinline__ void cp_async_wait()   // at most N of this thread's 
 #endif
 }
 
-template <int BPP>
-__device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_prev, uint32_t* prog_mine, uint4 (*ring)[32],
+// Where wave_band writes the pixels of a row: an ImageJob's go to PNG.Image.storage at stride pitch, a PassJob's over the
+// row's own filtered bytes, at stride pitch + 1 from offset 1.
+__device__ __forceinline__ uint8_t* wave_out(const ImageJob& job) { return job.pixels; }
+__device__ __forceinline__ uint32_t wave_out_stride(const ImageJob& job) { return job.pitch; }
+__device__ __forceinline__ uint8_t* wave_out(const PassJob& job) { return job.filtered + 1; }
+__device__ __forceinline__ uint32_t wave_out_stride(const PassJob& job) { return job.pitch + 1; }
+// Rows of the job the stream delivered in full (wave_band also stops at the job's height).  A pass starts `offset`
+// bytes into its image's stream: when the stream ends in front of it, or after an inflate error, it has none.
+__device__ __forceinline__ uint64_t wave_rows(const ImageJob& job, uint32_t pitch)
+{
+    return usable_bytes(job.inflated, job.filtered_len) / (pitch + 1);
+}
+__device__ __forceinline__ uint64_t wave_rows(const PassJob& job, uint32_t pitch)
+{
+    const uint64_t usable = usable_bytes(job.inflated, job.filtered_len);
+    return usable > job.offset ? (usable - job.offset) / (pitch + 1) : 0;
+}
+
+// Job is ImageJob or PassJob.  In place (PassJob), the rows of a job lie back to back, so the aligned 16-byte chunk a
+// lane stages first also holds the tail of the row above, and the last one it stages the head of the row below; lane 0
+// reading the band above's last row through load16_any reads the head of its own row with it.  Those neighbours may be
+// rewriting the bytes in the meantime: they lie outside the row and are read and discarded.  A lane's own input bytes
+// are never rewritten before they are read: output chunk j covers aligned input chunks j and j + 1, and it is stored
+// at step j or j + 1, after the ring has taken both (cp_async_wait below).
+template <int BPP, typename Job>
+__device__ void wave_band(const Job& job, uint32_t band, uint32_t* prog_prev, uint32_t* prog_mine, uint4 (*ring)[32],
                           unsigned long long* hist)
 {
+    constexpr bool in_place = std::is_same<Job, PassJob>::value;
     const unsigned lane   = lane_id();
     const uint32_t y      = band * 32 + lane;
     const uint32_t pitch  = job.pitch;
-    const uint64_t rows   = usable_bytes(job.inflated, job.filtered_len) / (pitch + 1);
+    const uint64_t rows   = wave_rows(job, pitch);
     const bool     active = y < job.height && y < rows;
     const int      nchunk = (int)((pitch + 15) >> 4);
     const uint8_t* row    = job.filtered + (uint64_t)(active ? y : 0) * (pitch + 1);
@@ -188,14 +232,17 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
     const uint32_t m     = (uint32_t)((uintptr_t)in & 15);
     const uint4*   inq   = (const uint4*)(in - m);
     const int      nq    = (int)(((uint64_t)m + pitch + 15) >> 4);  // aligned chunks that hold row bytes
-    uint8_t*       out   = job.pixels + (uint64_t)(active ? y : 0) * pitch;
-    const uint8_t* above = band == 0 ? nullptr : job.pixels + (uint64_t)(band * 32 - 1) * pitch;
+    uint8_t*       out   = wave_out(job) + (uint64_t)(active ? y : 0) * wave_out_stride(job);
+    const uint8_t* above = band == 0 ? nullptr : wave_out(job) + (uint64_t)(band * 32 - 1) * wave_out_stride(job);
     const bool     publish = lane == 31 && prog_mine != nullptr;
     // rows the stream did not deliver (a complete zlib stream that is shorter than the image is not an error in
-    // the reference: the rows simply stay as PNG.Image.storage was initialised, zero -- PNG.Image.swift:84)
-    if (!active && y < job.height) {
-        uint8_t* z = job.pixels + (uint64_t)y * pitch;
-        for (uint32_t k = 0; k < pitch; ++k) z[k] = 0;
+    // the reference: the rows simply stay as PNG.Image.storage was initialised, zero -- PNG.Image.swift:84).  In
+    // place they are left alone: unfilter_interleave_kernel writes their zeros, and the stream may end inside them.
+    if constexpr (!in_place) {
+        if (!active && y < job.height) {
+            uint8_t* z = job.pixels + (uint64_t)y * pitch;
+            for (uint32_t k = 0; k < pitch; ++k) z[k] = 0;
+        }
     }
 
     uint4    qcur  = make_uint4(0, 0, 0, 0);
@@ -314,7 +361,8 @@ __device__ void wave_band(const ImageJob& job, uint32_t band, uint32_t* prog_pre
     __syncwarp();
 }
 
-__global__ void __launch_bounds__(WAVE_WARPS * 32) unfilter_wave_kernel(WaveParams p)
+template <typename Job>
+__device__ __forceinline__ void wave_run(const WaveParams& p)
 {
     PNGB200_DYN_SMEM(wave_smem);   // [warp][slot][lane] input rings: conflict-free 16-byte accesses
     uint4 (*ring)[32] = reinterpret_cast<uint4 (*)[32]>(wave_smem) + (threadIdx.x >> 5) * WAVE_DEPTH;
@@ -347,7 +395,7 @@ __global__ void __launch_bounds__(WAVE_WARPS * 32) unfilter_wave_kernel(WavePara
             band = t - p.band_base[lo];
             gidx = t;
         }
-        const ImageJob job   = p.jobs[lo];
+        const Job      job   = static_cast<const Job*>(p.jobs)[lo];
         const uint32_t nband = p.band_base[lo + 1] - p.band_base[lo];
         uint32_t*      prev  = band == 0 ? nullptr : p.progress + gidx - 1;
         uint32_t*      mine  = band + 1 < nband ? p.progress + gidx : nullptr;
@@ -361,6 +409,11 @@ __global__ void __launch_bounds__(WAVE_WARPS * 32) unfilter_wave_kernel(WavePara
         }
     }
 }
+
+__global__ void __launch_bounds__(WAVE_WARPS * 32) unfilter_wave_kernel(WaveParams p) { wave_run<ImageJob>(p); }
+
+// p.hist must be null: the filter histogram counts the non-interlaced images of 8 bits or more only
+__global__ void __launch_bounds__(WAVE_WARPS * 32) unfilter_pass_kernel(WaveParams p) { wave_run<PassJob>(p); }
 
 // ---- generic path: Adam7 and sub-byte depths.  One CTA per image; defilters in place. ----
 __constant__ int c_adam7[7][4] = {{0, 0, 3, 3}, {4, 0, 3, 3}, {0, 4, 2, 3}, {2, 0, 2, 2},
@@ -440,6 +493,118 @@ __global__ void __launch_bounds__(128) unfilter_generic_kernel(const GenericJob*
             last = line;
             at += pitch + 1;
             __syncthreads();
+        }
+    }
+}
+
+// ---- the pass path's second kernel: PNG.Image.assign from the rows unfilter_pass_kernel reconstructed in place ----
+struct InterleaveJob {
+    const uint8_t*      filtered;      // the image's filtered stream, its passes reconstructed
+    uint8_t*            pixels;        // PNG.Image.storage
+    const StreamResult* inflated;      // may be null
+    uint64_t            filtered_len;  // used when `inflated` is null
+    uint64_t            block_base;    // the image's first CTA block of the launch
+    uint32_t            width, height;
+    uint8_t             volume, depth, interlaced, bpp;
+};
+
+constexpr int INTERLEAVE_THREADS = 256;   // one aligned 16-byte chunk of storage per thread and block
+
+// Every byte of an image's storage, in output order: a block writes 4 KiB that are contiguous in memory, a thread one
+// aligned 16-byte chunk of it with a single store, so that every store fills whole 32-byte sectors.  A pixel takes its
+// sample from its pass row (Adam7 origin and step per c_adam7; a 1/2/4-bit sample MSB-first, one byte per pixel), or
+// zero where that row was not reconstructed: storage starts out zeroed in the reference (PNG.Image.swift:84).  Rows
+// per pass follow wave_rows: the stream up to the first incomplete row, none after an inflate error.
+__global__ void __launch_bounds__(INTERLEAVE_THREADS) unfilter_interleave_kernel(const InterleaveJob* jobs, uint32_t count,
+                                                                                 uint64_t blocks)
+{
+    __shared__ const uint8_t* s_line[7];   // pixel bytes of the pass's row 0
+    __shared__ uint64_t       s_stride[7]; // pitch + 1
+    __shared__ uint64_t       s_rows[7];   // rows reconstructed
+    for (uint64_t b = blockIdx.x; b < blocks; b += gridDim.x) {
+        uint32_t lo = 0, hi = count;   // image owning block b: last index with block_base <= b
+        while (hi - lo > 1) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (jobs[mid].block_base <= b) lo = mid;
+            else hi = mid;
+        }
+        const InterleaveJob job = jobs[lo];
+        __syncthreads();   // the previous block's threads are done with the pass table
+        if (threadIdx.x < 7) {
+            const int z = threadIdx.x;
+            uint64_t  off = 0, sw = 0, sh = 0, pitch = 0;
+            for (int k = 0; k <= z; ++k) {   // the passes in front of z, then z itself
+                if (job.interlaced) {
+                    sw = ((uint64_t)job.width + (1u << c_adam7[k][2]) - c_adam7[k][0] - 1) >> c_adam7[k][2];
+                    sh = ((uint64_t)job.height + (1u << c_adam7[k][3]) - c_adam7[k][1] - 1) >> c_adam7[k][3];
+                } else {
+                    sw = k == 0 ? job.width : 0;
+                    sh = k == 0 ? job.height : 0;
+                }
+                pitch = (sw * job.volume + 7) >> 3;
+                if (k < z && sw != 0) off += sh * (pitch + 1);
+            }
+            const uint64_t usable = usable_bytes(job.inflated, job.filtered_len);
+            const uint64_t rows   = usable > off && sw != 0 ? (usable - off) / (pitch + 1) : 0;
+            s_line[z]   = job.filtered + off + 1;
+            s_stride[z] = pitch + 1;
+            s_rows[z]   = rows < sh ? rows : sh;
+        }
+        __syncthreads();
+        const uint32_t bpp   = job.bpp;
+        const uint32_t lper  = job.depth == 1 ? 3 : job.depth == 2 ? 2 : 1;
+        const uint64_t bytes = (uint64_t)job.width * job.height * bpp;
+        const uint32_t mis   = (uint32_t)((uintptr_t)job.pixels & 15);
+        // chunk k of the image covers storage bytes [16 k - mis, 16 k - mis + 16)
+        const uint64_t k     = (b - job.block_base) * INTERLEAVE_THREADS + threadIdx.x;
+        const int64_t  first = (int64_t)(16 * k) - mis;
+        if (first >= (int64_t)bytes) continue;
+        const uint64_t s  = first < 0 ? 0 : (uint64_t)first;
+        const uint64_t e  = min((uint64_t)(first + 16), bytes);
+        const uint64_t px = s / bpp;
+        uint32_t       c  = (uint32_t)(s - px * bpp);
+        uint64_t       y  = px / job.width;
+        uint32_t       x  = (uint32_t)(px - y * job.width);
+        uint32_t       w0 = 0, w1 = 0, w2 = 0, w3 = 0;
+        for (uint64_t at = s; at < e; ++at) {
+            int z = 0;   // Adam7 pass of pixel (x, y)
+            if (job.interlaced)
+                z = (y & 1) ? 6 : (x & 1) ? 5 : (y & 2) ? 4 : (x & 2) ? 3 : (y & 4) ? 2 : (x & 4) ? 1 : 0;
+            const int      ex = job.interlaced ? c_adam7[z][2] : 0, ey = job.interlaced ? c_adam7[z][3] : 0;
+            const uint64_t r  = y >> ey;   // (y - origin) >> step: the origin's bits sit below the step
+            const uint64_t i  = x >> ex;
+            uint32_t       v  = 0;
+            if (r < s_rows[z]) {
+                const uint8_t* line = s_line[z] + r * s_stride[z];
+                if (job.depth < 8) {   // 1, 2 or 4 bits: 8 >> lper samples a byte
+                    const uint32_t sh = ((~(uint32_t)i) & ((1u << lper) - 1)) * job.depth;
+                    v = (line[i >> lper] >> sh) & ((1u << job.depth) - 1);
+                } else {
+                    v = line[i * bpp + c];
+                }
+            }
+            const uint32_t slot = (uint32_t)(at - (uint64_t)first), sv = v << (8 * (slot & 3));
+            w0 |= slot < 4 ? sv : 0u;   // selects, not w[slot >> 2]: a dynamically indexed array goes to local memory
+            w1 |= slot >> 2 == 1 ? sv : 0u;
+            w2 |= slot >> 2 == 2 ? sv : 0u;
+            w3 |= slot >= 12 ? sv : 0u;
+            if (++c == bpp) {
+                c = 0;
+                if (++x == job.width) {
+                    x = 0;
+                    ++y;
+                }
+            }
+        }
+        uint8_t* dst = job.pixels + (int64_t)first;   // aligned: 16 k - mis bytes past the start of the storage
+        if (first >= 0 && e - s == 16) {
+            *(uint4*)dst = make_uint4(w0, w1, w2, w3);
+        } else {   // the image's first or last chunk
+            for (uint64_t at = s; at < e; ++at) {
+                const uint32_t slot = (uint32_t)(at - (uint64_t)first);
+                const uint32_t word = slot < 4 ? w0 : slot < 8 ? w1 : slot < 12 ? w2 : w3;
+                job.pixels[at] = (uint8_t)(word >> (8 * (slot & 3)));
+            }
         }
     }
 }
