@@ -94,9 +94,6 @@ struct Slots {
     }
 };
 
-const int ADAM7[7][4] = {{0, 0, 3, 3}, {4, 0, 3, 3}, {0, 4, 2, 3}, {2, 0, 2, 2},
-                         {0, 2, 1, 2}, {1, 0, 1, 1}, {0, 1, 0, 1}};
-
 }  // namespace
 
 struct pngb200_ctx {
@@ -799,88 +796,18 @@ struct UnfilterItem {
 // per image spends on its rows (DESIGN §4.3, the size sweep of tools/unfilter_passes_bw.py).
 constexpr uint64_t UNFILTER_GENERIC_MAX = 65536;
 
-// The wavefront's ticket order over `jobs` (ImageJob or PassJob, `height` rows each).  Tickets go out band level by band
-// level (see WaveParams): jobs sorted by band count, descending; level_start[b] = tickets in front of level b.  (Jobs of
-// more than 4096 bands -- 131072 rows -- keep the job-major order and leave level_start empty.)  band_base[i] = the
-// first band of job i.  Returns the number of bands.
-template <typename Job>
-uint64_t plan_bands(std::vector<Job>& jobs, std::vector<uint32_t>& band_base, std::vector<uint32_t>& level_start)
-{
-    auto nb = [&](const Job& j) { return (j.height + 31) / 32; };
-    level_start.clear();
-    std::vector<uint32_t> idx(jobs.size());
-    for (size_t i = 0; i < idx.size(); ++i) idx[i] = (uint32_t)i;
-    std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return nb(jobs[a]) > nb(jobs[b]); });
-    const uint32_t maxb = jobs.empty() ? 0 : nb(jobs[idx[0]]);
-    if (!jobs.empty() && maxb <= 4096) {
-        std::vector<Job> sorted(jobs.size());
-        for (size_t i = 0; i < idx.size(); ++i) sorted[i] = jobs[idx[i]];
-        jobs.swap(sorted);
-        level_start.assign(maxb + 1, 0);
-        size_t alive = jobs.size();          // jobs with more than b bands: a prefix of the sorted list
-        for (uint32_t b = 0; b < maxb; ++b) {
-            while (alive && nb(jobs[alive - 1]) <= b) --alive;
-            level_start[b + 1] = level_start[b] + (uint32_t)alive;
-        }
-    }
-    band_base.assign(jobs.size() + 1, 0);
-    uint64_t bands = 0;
-    for (size_t i = 0; i < jobs.size(); ++i) {
-        band_base[i] = (uint32_t)std::min<uint64_t>(bands, UINT32_MAX);
-        bands += nb(jobs[i]);
-    }
-    band_base[jobs.size()] = (uint32_t)std::min<uint64_t>(bands, UINT32_MAX);
-    return bands;
-}
-
 int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
 {
     ctx->d_hist = nullptr;
 
-    std::vector<ImageJob>   fast;
-    std::vector<GenericJob> slow;
-    std::vector<PassJob>    pass;
+    std::vector<ImageJob>      fast;
+    std::vector<GenericJob>    slow;
     std::vector<InterleaveJob> inter;
-    std::vector<uint32_t>   band_base;
-    uint64_t                inter_blocks = 0;
+    std::vector<PassJob>       pass;
+    std::vector<uint32_t>      band_base;
+    uint64_t                   inter_blocks = 0;
     for (const UnfilterItem& it : items) {
-        if (it.g.passes && it.g.filtered > UNFILTER_GENERIC_MAX) {
-            // one job per non-empty Adam7 pass, or one for a non-interlaced 1/2/4-bit image, at its offset in the stream
-            uint64_t off = 0;
-            for (int z = 0; z < (it.interlaced ? 7 : 1); ++z) {
-                uint64_t sw = it.w, sh = it.h;
-                if (it.interlaced) {
-                    sw = ((uint64_t)it.w + (1u << ADAM7[z][2]) - ADAM7[z][0] - 1) >> ADAM7[z][2];
-                    sh = ((uint64_t)it.h + (1u << ADAM7[z][3]) - ADAM7[z][1] - 1) >> ADAM7[z][3];
-                    if (sw == 0 || sh == 0) continue;
-                }
-                PassJob j;
-                j.pitch = (uint32_t)((sw * it.volume + 7) >> 3);
-                j.filtered = it.filtered_mut + off;
-                j.inflated = it.inflated;
-                j.filtered_len = it.filtered_len;
-                j.offset = off;
-                j.height = (uint32_t)sh;
-                j.bpp = it.g.bpp;
-                pass.push_back(j);
-                off += sh * ((uint64_t)j.pitch + 1);
-            }
-            InterleaveJob j;
-            j.filtered = it.filtered_mut;
-            j.pixels = it.pixels;
-            j.inflated = it.inflated;
-            j.filtered_len = it.filtered_len;
-            j.block_base = inter_blocks;
-            j.width = it.w;
-            j.height = it.h;
-            j.volume = it.volume;
-            j.depth = it.depth;
-            j.interlaced = it.interlaced;
-            j.bpp = it.g.bpp;
-            inter.push_back(j);
-            const uint64_t chunks = (15 + it.g.storage + 15) / 16;   // any misalignment of the pixels
-            inter_blocks += (chunks + INTERLEAVE_THREADS - 1) / INTERLEAVE_THREADS;
-        } else if (it.g.fast) {
+        if (it.g.fast) {
             ImageJob j;
             j.filtered = it.filtered;
             j.pixels = it.pixels;
@@ -894,20 +821,22 @@ int run_unfilter(pngb200_ctx* ctx, const std::vector<UnfilterItem>& items)
             j.interlaced = 0;
             j.bpp = it.g.bpp;
             fast.push_back(j);
-        } else {
-            GenericJob j;
-            j.filtered = it.filtered_mut;
-            j.pixels = it.pixels;
-            j.inflated = it.inflated;
-            j.filtered_len = it.filtered_len;
-            j.width = it.w;
-            j.height = it.h;
-            j.volume = it.volume;
-            j.depth = it.depth;
-            j.interlaced = it.interlaced;
-            j.bpp = it.g.bpp;
-            slow.push_back(j);
+            continue;
         }
+        PassImageJob j;
+        j.filtered = it.filtered_mut;
+        j.pixels = it.pixels;
+        j.inflated = it.inflated;
+        j.filtered_len = it.filtered_len;
+        j.block_base = 0;
+        j.width = it.w;
+        j.height = it.h;
+        j.volume = it.volume;
+        j.depth = it.depth;
+        j.interlaced = it.interlaced;
+        j.bpp = it.g.bpp;
+        if (it.g.passes && it.g.filtered > UNFILTER_GENERIC_MAX) plan_passes(j, pass, inter, inter_blocks);
+        else slow.push_back(j);
     }
     // the fast and the pass path hand out their bands level by level
     std::vector<uint32_t> level_start, pass_base, pass_levels;
@@ -1059,15 +988,7 @@ extern "C" {
 
 size_t pngb200_filtered_size(uint32_t w, uint32_t h, int volume, int interlaced)
 {
-    if (!interlaced) return (size_t)h * ((((size_t)w * (size_t)volume + 7) >> 3) + 1);
-    size_t total = 0;
-    for (int z = 0; z < 7; ++z) {
-        size_t sx = ((size_t)w + (1u << ADAM7[z][2]) - ADAM7[z][0] - 1) >> ADAM7[z][2];
-        size_t sy = ((size_t)h + (1u << ADAM7[z][3]) - ADAM7[z][1] - 1) >> ADAM7[z][3];
-        if (sx == 0 || sy == 0) continue;
-        total += sy * (((sx * (size_t)volume + 7) >> 3) + 1);
-    }
-    return total;
+    return stream_pass_offset(7, w, h, (size_t)volume, interlaced);
 }
 
 size_t pngb200_storage_size(uint32_t w, uint32_t h, int volume)

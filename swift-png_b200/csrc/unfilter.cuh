@@ -25,7 +25,9 @@
 // unfilter_generic_kernel: the same formats when the filtered stream is short; one CTA per image.
 #pragma once
 
+#include <algorithm>
 #include <type_traits>
+#include <vector>
 
 #include "common.cuh"
 
@@ -115,6 +117,55 @@ __device__ __forceinline__ void store16_partial(uint8_t* p, uint4 v, int nbytes)
     } else {
         for (int i = 0; i < nbytes && i < 16; ++i) p[i] = (uint8_t)(w[i >> 2] >> (8 * (i & 3)));
     }
+}
+
+// ---- the layout of a filtered stream, shared by every scanline kernel and the host ----
+// Adam7 (PNG.adam7, PNG.Decoder.swift:6-15): pass z holds the pixels (bx + (i << ex), by + (r << ey)), as
+// {bx, by, ex, ey}.  The host reads h_adam7, the device its copy in constant memory.  The copy is defined here, after
+// the inflate and deflate tables (huffman.cuh, deflate.cuh), so that it does not move their constant-bank addresses.
+struct Adam7Table {
+    int p[7][4];
+};
+constexpr Adam7Table h_adam7 = {{{0, 0, 3, 3}, {4, 0, 3, 3}, {0, 4, 2, 3}, {2, 0, 2, 2}, {0, 2, 1, 2}, {1, 0, 1, 1}, {0, 1, 0, 1}}};
+__constant__ Adam7Table c_adam7 = h_adam7;
+
+// One pass of a filtered stream: Adam7 pass z of an interlaced image, or for z = 0 the whole of a non-interlaced one,
+// whose passes 1 to 6 are empty.  Its rows lie back to back, each a filter byte and `pitch` bytes; an empty Adam7 pass
+// has width = height = 0.  Sizes are 64-bit: a pass's width * volume passes 2^32 long before geometry()'s limits.
+struct Pass {
+    uint32_t bx, by, ex, ey;  // row r holds the pixels (bx + (i << ex), by + (r << ey)), i < width
+    uint64_t width, height;   // pixels per row, rows
+    uint64_t pitch;           // bytes per row, not counting the filter byte
+};
+
+__host__ __device__ __forceinline__ Pass stream_pass(int z, uint32_t w, uint32_t h, uint64_t volume, bool interlaced)
+{
+    Pass s = {0, 0, 0, 0, z == 0 ? w : 0u, z == 0 ? h : 0u, 0};
+    if (interlaced) {
+#ifdef __CUDA_ARCH__
+        const int* a = c_adam7.p[z];
+#else
+        const int* a = h_adam7.p[z];
+#endif
+        s.bx = a[0]; s.by = a[1]; s.ex = a[2]; s.ey = a[3];
+        s.width  = ((uint64_t)w + (1u << s.ex) - s.bx - 1) >> s.ex;
+        s.height = ((uint64_t)h + (1u << s.ey) - s.by - 1) >> s.ey;
+        if (s.width == 0 || s.height == 0) s.width = s.height = 0;
+    }
+    s.pitch = (s.width * volume + 7) >> 3;
+    return s;
+}
+
+// bytes of the filtered stream in front of pass z; z = 7 gives the length of the whole stream.  The loop has a fixed
+// trip count so that the compiler unrolls it: a loop up to z costs unfilter_interleave_kernel 8 more registers.
+__host__ __device__ __forceinline__ uint64_t stream_pass_offset(int z, uint32_t w, uint32_t h, uint64_t volume, bool interlaced)
+{
+    uint64_t off = 0;
+    for (int k = 0; k < 7; ++k) {
+        const Pass s = stream_pass(k, w, h, volume, interlaced);
+        if (k < z) off += s.height * (s.pitch + 1);
+    }
+    return off;
 }
 
 // One Adam7 pass of an image, or the whole of a non-interlaced 1/2/4-bit image, for unfilter_pass_kernel.  Its rows are
@@ -415,19 +466,21 @@ __global__ void __launch_bounds__(WAVE_WARPS * 32) unfilter_wave_kernel(WavePara
 // p.hist must be null: the filter histogram counts the non-interlaced images of 8 bits or more only
 __global__ void __launch_bounds__(WAVE_WARPS * 32) unfilter_pass_kernel(WaveParams p) { wave_run<PassJob>(p); }
 
-// ---- generic path: Adam7 and sub-byte depths.  One CTA per image; defilters in place. ----
-__constant__ int c_adam7[7][4] = {{0, 0, 3, 3}, {4, 0, 3, 3}, {0, 4, 2, 3}, {2, 0, 2, 2},
-                                  {0, 2, 1, 2}, {1, 0, 1, 1}, {0, 1, 0, 1}};
-
-struct GenericJob {
-    uint8_t*            filtered;  // mutable: rows are reconstructed in place
-    uint8_t*            pixels;
-    const StreamResult* inflated;
-    uint64_t            filtered_len;
-    uint32_t width, height;
-    uint8_t  volume, depth, interlaced, bpp;
+// An Adam7 or 1/2/4-bit image for unfilter_generic_kernel, which reconstructs its rows in place and assigns them, or
+// for unfilter_interleave_kernel, which assigns the passes unfilter_pass_kernel reconstructed in place.
+struct PassImageJob {
+    uint8_t*            filtered;      // the image's private (mutable) filtered stream
+    uint8_t*            pixels;        // PNG.Image.storage
+    const StreamResult* inflated;      // may be null
+    uint64_t            filtered_len;  // used when `inflated` is null
+    uint64_t            block_base;    // the image's first CTA block of the launch (unfilter_interleave_kernel only)
+    uint32_t            width, height;
+    uint8_t             volume, depth, interlaced, bpp;
 };
+using GenericJob    = PassImageJob;   // each kernel's name for its job
+using InterleaveJob = PassImageJob;
 
+// ---- generic path: Adam7 and sub-byte depths.  One CTA per image; defilters in place. ----
 __global__ void __launch_bounds__(128) unfilter_generic_kernel(const GenericJob* jobs, int count)
 {
     if ((int)blockIdx.x >= count) return;
@@ -442,19 +495,11 @@ __global__ void __launch_bounds__(128) unfilter_generic_kernel(const GenericJob*
         __syncthreads();
     }
     const uint8_t*   end = job.filtered + usable_bytes(job.inflated, job.filtered_len);
-    const int npass = job.interlaced ? 7 : 1;
-    for (int z = 0; z < npass; ++z) {
-        int      bx = 0, by = 0, ex = 0, ey = 0;
-        uint32_t sw = job.width, shh = job.height;
-        if (job.interlaced) {
-            bx = c_adam7[z][0]; by = c_adam7[z][1]; ex = c_adam7[z][2]; ey = c_adam7[z][3];
-            sw  = (job.width + (1u << ex) - bx - 1) >> ex;
-            shh = (job.height + (1u << ey) - by - 1) >> ey;
-            if (sw == 0 || shh == 0) continue;
-        }
-        // sw * volume passes 2^32 from sw = 2^26 (RGBA16) on: the pitch is computed in 64 bits (it fits 32 again, as
-        // geometry() caps it at 0xfffffff0), and the byte loops below count in 64 bits so that i + nt cannot wrap
-        const uint32_t pitch = (uint32_t)(((uint64_t)sw * job.volume + 7) >> 3);
+    for (int z = 0; z < 7; ++z) {
+        const Pass ps = stream_pass(z, job.width, job.height, job.volume, job.interlaced);
+        // the pitch fits 32 bits (geometry() caps it at 0xfffffff0); the byte loops below count in 64 bits so that
+        // i + nt cannot wrap
+        const uint32_t sw = (uint32_t)ps.width, shh = (uint32_t)ps.height, pitch = (uint32_t)ps.pitch;
         uint8_t*       last  = nullptr;
         for (uint32_t y = 0; y < shh; ++y) {
             if (at + pitch + 1 > end) return;  // inflator.pull(pitch + 1) == nil
@@ -476,18 +521,18 @@ __global__ void __launch_bounds__(128) unfilter_generic_kernel(const GenericJob*
             }
             __syncthreads();
             // PNG.Image.assign
-            const uint32_t oy = by + (y << ey);
+            const uint32_t oy = ps.by + (y << ps.ey);
             if (job.depth < 8) {
                 const uint32_t per = 8 / job.depth, mask = (1u << job.depth) - 1;
                 for (uint32_t i = tid; i < sw; i += nt) {
                     uint32_t sh = ((~i) & (per - 1)) * job.depth;
-                    job.pixels[(uint64_t)oy * job.width + bx + ((uint64_t)i << ex)] =
+                    job.pixels[(uint64_t)oy * job.width + ps.bx + ((uint64_t)i << ps.ex)] =
                         (uint8_t)((line[i / per] >> sh) & mask);
                 }
             } else {
                 for (uint64_t k = tid; k < pitch; k += nt) {   // depth >= 8: sw * bpp == pitch
                     uint32_t i = (uint32_t)k / bpp, c = (uint32_t)k - i * bpp;
-                    job.pixels[((uint64_t)oy * job.width + bx + ((uint64_t)i << ex)) * bpp + c] = line[k];
+                    job.pixels[((uint64_t)oy * job.width + ps.bx + ((uint64_t)i << ps.ex)) * bpp + c] = line[k];
                 }
             }
             last = line;
@@ -498,16 +543,6 @@ __global__ void __launch_bounds__(128) unfilter_generic_kernel(const GenericJob*
 }
 
 // ---- the pass path's second kernel: PNG.Image.assign from the rows unfilter_pass_kernel reconstructed in place ----
-struct InterleaveJob {
-    const uint8_t*      filtered;      // the image's filtered stream, its passes reconstructed
-    uint8_t*            pixels;        // PNG.Image.storage
-    const StreamResult* inflated;      // may be null
-    uint64_t            filtered_len;  // used when `inflated` is null
-    uint64_t            block_base;    // the image's first CTA block of the launch
-    uint32_t            width, height;
-    uint8_t             volume, depth, interlaced, bpp;
-};
-
 constexpr int INTERLEAVE_THREADS = 256;   // one aligned 16-byte chunk of storage per thread and block
 
 // Every byte of an image's storage, in output order: a block writes 4 KiB that are contiguous in memory, a thread one
@@ -531,24 +566,14 @@ __global__ void __launch_bounds__(INTERLEAVE_THREADS) unfilter_interleave_kernel
         const InterleaveJob job = jobs[lo];
         __syncthreads();   // the previous block's threads are done with the pass table
         if (threadIdx.x < 7) {
-            const int z = threadIdx.x;
-            uint64_t  off = 0, sw = 0, sh = 0, pitch = 0;
-            for (int k = 0; k <= z; ++k) {   // the passes in front of z, then z itself
-                if (job.interlaced) {
-                    sw = ((uint64_t)job.width + (1u << c_adam7[k][2]) - c_adam7[k][0] - 1) >> c_adam7[k][2];
-                    sh = ((uint64_t)job.height + (1u << c_adam7[k][3]) - c_adam7[k][1] - 1) >> c_adam7[k][3];
-                } else {
-                    sw = k == 0 ? job.width : 0;
-                    sh = k == 0 ? job.height : 0;
-                }
-                pitch = (sw * job.volume + 7) >> 3;
-                if (k < z && sw != 0) off += sh * (pitch + 1);
-            }
+            const int      z      = threadIdx.x;
+            const Pass     ps     = stream_pass(z, job.width, job.height, job.volume, job.interlaced);
+            const uint64_t off    = stream_pass_offset(z, job.width, job.height, job.volume, job.interlaced);
             const uint64_t usable = usable_bytes(job.inflated, job.filtered_len);
-            const uint64_t rows   = usable > off && sw != 0 ? (usable - off) / (pitch + 1) : 0;
+            const uint64_t rows   = usable > off ? (usable - off) / (ps.pitch + 1) : 0;
             s_line[z]   = job.filtered + off + 1;
-            s_stride[z] = pitch + 1;
-            s_rows[z]   = rows < sh ? rows : sh;
+            s_stride[z] = ps.pitch + 1;
+            s_rows[z]   = rows < ps.height ? rows : ps.height;
         }
         __syncthreads();
         const uint32_t bpp   = job.bpp;
@@ -570,7 +595,7 @@ __global__ void __launch_bounds__(INTERLEAVE_THREADS) unfilter_interleave_kernel
             int z = 0;   // Adam7 pass of pixel (x, y)
             if (job.interlaced)
                 z = (y & 1) ? 6 : (x & 1) ? 5 : (y & 2) ? 4 : (x & 2) ? 3 : (y & 4) ? 2 : (x & 4) ? 1 : 0;
-            const int      ex = job.interlaced ? c_adam7[z][2] : 0, ey = job.interlaced ? c_adam7[z][3] : 0;
+            const int      ex = job.interlaced ? c_adam7.p[z][2] : 0, ey = job.interlaced ? c_adam7.p[z][3] : 0;
             const uint64_t r  = y >> ey;   // (y - origin) >> step: the origin's bits sit below the step
             const uint64_t i  = x >> ex;
             uint32_t       v  = 0;
@@ -607,6 +632,59 @@ __global__ void __launch_bounds__(INTERLEAVE_THREADS) unfilter_interleave_kernel
             }
         }
     }
+}
+
+// ---- host planning of the wavefront and the pass path ----
+
+// The wavefront's ticket order over `jobs` (ImageJob or PassJob, `height` rows each).  Tickets go out band level by band
+// level (see WaveParams): jobs sorted by band count, descending; level_start[b] = tickets in front of level b.  (Jobs of
+// more than 4096 bands -- 131072 rows -- keep the job-major order and leave level_start empty.)  band_base[i] = the
+// first band of job i.  Returns the number of bands.
+template <typename Job>
+uint64_t plan_bands(std::vector<Job>& jobs, std::vector<uint32_t>& band_base, std::vector<uint32_t>& level_start)
+{
+    auto nb = [&](const Job& j) { return (j.height + 31) / 32; };
+    level_start.clear();
+    std::vector<uint32_t> idx(jobs.size());
+    for (size_t i = 0; i < idx.size(); ++i) idx[i] = (uint32_t)i;
+    std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return nb(jobs[a]) > nb(jobs[b]); });
+    const uint32_t maxb = jobs.empty() ? 0 : nb(jobs[idx[0]]);
+    if (!jobs.empty() && maxb <= 4096) {
+        std::vector<Job> sorted(jobs.size());
+        for (size_t i = 0; i < idx.size(); ++i) sorted[i] = jobs[idx[i]];
+        jobs.swap(sorted);
+        level_start.assign(maxb + 1, 0);
+        size_t alive = jobs.size();          // jobs with more than b bands: a prefix of the sorted list
+        for (uint32_t b = 0; b < maxb; ++b) {
+            while (alive && nb(jobs[alive - 1]) <= b) --alive;
+            level_start[b + 1] = level_start[b] + (uint32_t)alive;
+        }
+    }
+    band_base.assign(jobs.size() + 1, 0);
+    uint64_t bands = 0;
+    for (size_t i = 0; i < jobs.size(); ++i) {
+        band_base[i] = (uint32_t)std::min<uint64_t>(bands, UINT32_MAX);
+        bands += nb(jobs[i]);
+    }
+    band_base[jobs.size()] = (uint32_t)std::min<uint64_t>(bands, UINT32_MAX);
+    return bands;
+}
+
+// The pass path's work for one image: a PassJob per non-empty pass, reconstructed in place in `image.filtered`, then
+// the image itself for unfilter_interleave_kernel, its blocks numbered from `blocks` on (advanced past them).
+inline void plan_passes(InterleaveJob image, std::vector<PassJob>& passes, std::vector<InterleaveJob>& images, uint64_t& blocks)
+{
+    for (int z = 0; z < 7; ++z) {
+        const Pass ps = stream_pass(z, image.width, image.height, image.volume, image.interlaced);
+        if (ps.height == 0) continue;
+        const uint64_t off = stream_pass_offset(z, image.width, image.height, image.volume, image.interlaced);
+        passes.push_back({image.filtered + off, image.inflated, image.filtered_len, off, (uint32_t)ps.height,
+                          (uint32_t)ps.pitch, image.bpp});
+    }
+    image.block_base = blocks;
+    images.push_back(image);
+    const uint64_t chunks = (15 + (uint64_t)image.width * image.height * image.bpp + 15) / 16;   // any misalignment of the pixels
+    blocks += (chunks + INTERLEAVE_THREADS - 1) / INTERLEAVE_THREADS;
 }
 
 }  // namespace pngb200

@@ -22,35 +22,25 @@ extern "C" int emu_unfilter(const uint8_t* filtered, uint64_t filtered_len, uint
     simt::launch(grid, WAVE_WARPS * 32, WAVE_SMEM, [&]() { unfilter_wave_kernel(p); }, order, true);
     return 0;
 }
-// several images (sorted by height, descending, as run_unfilter does), tickets level by level
+// several images, planned by plan_bands as run_unfilter plans them: tickets level by level, or job by job past 4096 bands
 extern "C" int emu_unfilter_multi(int n, const uint8_t* const* filtered, const uint64_t* filtered_len, uint8_t* const* pixels,
                                   const uint32_t* w, const uint32_t* h, uint32_t bpp, uint32_t depth, unsigned grid, int order)
 {
     std::vector<ImageJob> jobs(n);
-    std::vector<uint32_t> band_base(n + 1, 0);
-    uint32_t maxb = 0;
     for (int i = 0; i < n; ++i) {
         ImageJob& job = jobs[i];
         job = ImageJob{};
         job.filtered = filtered[i]; job.pixels = pixels[i]; job.inflated = nullptr; job.filtered_len = filtered_len[i];
         job.width = w[i]; job.height = h[i]; job.pitch = w[i] * bpp; job.volume = (uint8_t)(8 * bpp); job.depth = (uint8_t)depth;
         job.interlaced = 0; job.bpp = (uint8_t)bpp;
-        band_base[i + 1] = band_base[i] + (h[i] + 31) / 32;
-        maxb = std::max(maxb, (h[i] + 31) / 32);
     }
-    std::vector<uint32_t> level_start(maxb + 1, 0);
-    for (uint32_t b = 0; b < maxb; ++b) {
-        uint32_t alive = 0;
-        for (int i = 0; i < n; ++i) alive += (h[i] + 31) / 32 > b;
-        level_start[b + 1] = level_start[b] + alive;
-    }
-    const uint32_t bands = band_base[n];
+    std::vector<uint32_t> band_base, level_start;
+    const uint32_t bands = (uint32_t)plan_bands(jobs, band_base, level_start);
     std::vector<uint32_t> progress(bands + 1, 0);
-    uint32_t ticket = 0;
     WaveParams p{};
-    p.jobs = jobs.data(); p.band_base = band_base.data(); p.progress = progress.data(); p.ticket = &ticket;
+    p.jobs = jobs.data(); p.band_base = band_base.data(); p.progress = progress.data(); p.ticket = &progress[bands];
     p.njobs = (uint32_t)n; p.total_bands = bands; p.hist = nullptr;
-    p.level_start = level_start.data(); p.levels = maxb;
+    p.level_start = level_start.data(); p.levels = level_start.empty() ? 0u : (uint32_t)level_start.size() - 1;
     simt::launch(grid, WAVE_WARPS * 32, WAVE_SMEM, [&]() { unfilter_wave_kernel(p); }, order, true);
     return 0;
 }
