@@ -425,6 +425,49 @@ size_t pngb200_inflator_pull_all(pngb200_inflator* z, uint8_t* dst, size_t cap);
 size_t pngb200_inflator_available(const pngb200_inflator* z);
 void   pngb200_inflator_error(const pngb200_inflator* z, int* status, uint32_t* a, uint32_t* b);
 
+/* ---- online decoding: PNG.Context (Sources/PNG/Decoding/PNG.Context.swift) ----------------------------------------
+ * A caller pushes each IDAT chunk as it arrives; after every push the storage is a valid partial image.  Restates
+ * PNG.Context.push(data:overdraw:), the row state machine of PNG.Decoder.push (PNG.Decoder.swift:47-149),
+ * PNG.Image.assign and PNG.Image.overdraw (PNG.Image.swift:133-285), and push(ancillary:) with IEND.
+ * Inflate runs on the device through a pngb200_inflator; the newly available scanlines are reconstructed by
+ * unfilter_pass_kernel and written into storage, pass by pass, by context_assign_kernel.  After each push the rows
+ * assigned are exactly the reference's: its inflator releases the payload of a stored block as it arrives, and so
+ * does the context (the pngb200_inflator handle itself waits for the whole block). */
+typedef struct pngb200_png_context pngb200_png_context;
+typedef struct pngb200_png_context_desc {
+    void*    pixels;       /* PNG.Image.storage, width*height*((volume+7)>>3) bytes, in `memspace`; any alignment */
+    size_t   pixels_cap;
+    uint32_t width, height;
+    uint8_t  volume, depth, interlaced, standard;   /* standard 0 common (zlib), 1 ios (raw deflate) */
+    int32_t  memspace;     /* pngb200_memspace */
+} pngb200_png_context_desc;
+/* PNG.Context.init(..., uninitialized: false): zero-fills the storage (with `uninitialized: true` the reference leaves
+ * unassigned bytes undefined; zero is one of the values they may have).  Bad geometry or pixel format, too small a
+ * pixels_cap, an unknown standard or memspace: NULL, and pngb200_last_error says why. */
+pngb200_png_context* pngb200_png_context_create(pngb200_ctx* ctx, const pngb200_png_context_desc* desc);
+/* push(data:overdraw:) with host `data` (one IDAT payload, any length, empty included).  Returns PNGB200_OK, or:
+ *   PNGB200_ERR_PNG_EXTRANEOUS_COMPRESSED_DATA  the stream was already complete (even for an empty push);
+ *   an inflate error, with the reference's payload in pngb200_png_context_error: no row of the failing push is
+ *     assigned, storage stays as the previous push left it, and every later push returns the same error (the
+ *     reference leaves its state after a throw unspecified; this is one consistent choice);
+ *   PNGB200_ERR_PNG_EXTRANEOUS_IMAGE_DATA  every row is assigned and filtered bytes remain, in the push that
+ *     completes the image or in any later one that brings more; the rows are still assigned;
+ *   PNGB200_ERR_BAD_ARGUMENT while a decode batch is pending on the ctx.
+ * Otherwise every complete scanline now available is reconstructed and assigned in pass order, resuming mid-pass; with
+ * `overdraw` each scanline is overdrawn right after it is assigned (it may differ from one push to the next).  The call
+ * returns once the storage holds the new rows, host or device. */
+int  pngb200_png_context_push(pngb200_png_context* c, const uint8_t* data, size_t n, int overdraw);
+/* push(ancillary:) with IEND: PNGB200_OK if and only if the DEFLATE stream is complete, else
+ * PNGB200_ERR_PNG_INCOMPLETE_DATASTREAM.  A complete stream with too few rows is OK, as in pngb200_decode_batch. */
+int  pngb200_png_context_end(pngb200_png_context* c);
+/* out[0] next pass (0-6), 7 once every row is assigned (a non-interlaced image reports 0, then 7: PNG.Decoder.pass);
+ * out[1] next row of that pass; out[2] filtered bytes consumed; out[3] 1 once the stream is complete; out[4], out[5]
+ * the first storage row the last push wrote and one past its last (0, 0 if none): the band a viewer redraws. */
+int  pngb200_png_context_progress(const pngb200_png_context* c, uint64_t out[6]);
+/* the sticky inflate error (PNGB200_OK if none) and its payload */
+void pngb200_png_context_error(const pngb200_png_context* c, int* status, uint32_t* a, uint32_t* b);
+void pngb200_png_context_destroy(pngb200_png_context* c);
+
 /* LZ77.Deflator value-type semantics (Sources/LZ77/Deflator/LZ77.Deflator.swift:8-44; the call sites are
  * PNG.Encoder.pull, Sources/PNG/Encoding/PNG.Encoder.swift:68,85,101,117,121,128).
  * init(format:level:exponent:hint:) -- `chunk_bytes` is the size of a complete output block: the reference hands out

@@ -170,6 +170,14 @@ class PngEncodeDesc(C.Structure):
     ]
 
 
+class PngContextDesc(C.Structure):
+    _fields_ = [
+        ("pixels", C.c_void_p), ("pixels_cap", C.c_size_t), ("width", C.c_uint32), ("height", C.c_uint32),
+        ("volume", C.c_uint8), ("depth", C.c_uint8), ("interlaced", C.c_uint8), ("standard", C.c_uint8),
+        ("memspace", C.c_int32),
+    ]
+
+
 class PNGB200Error(RuntimeError):
     def __init__(self, status: int, message: str = ""):
         super().__init__(f"pngb200 status {status}: {message}")
@@ -292,6 +300,20 @@ def lib():
     L.pngb200_inflator_error.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_uint32),
                                          C.POINTER(C.c_uint32)]
     L.pngb200_inflator_error.restype = None
+    if os.environ.get("PNGB200_LIB") is None or hasattr(L, "pngb200_png_context_create"):   # (older builds lack it)
+        L.pngb200_png_context_create.argtypes = [C.c_void_p, C.POINTER(PngContextDesc)]
+        L.pngb200_png_context_create.restype = C.c_void_p
+        L.pngb200_png_context_push.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.c_int]
+        L.pngb200_png_context_push.restype = C.c_int
+        L.pngb200_png_context_end.argtypes = [C.c_void_p]
+        L.pngb200_png_context_end.restype = C.c_int
+        L.pngb200_png_context_progress.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.pngb200_png_context_progress.restype = C.c_int
+        L.pngb200_png_context_error.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_uint32),
+                                                C.POINTER(C.c_uint32)]
+        L.pngb200_png_context_error.restype = None
+        L.pngb200_png_context_destroy.argtypes = [C.c_void_p]
+        L.pngb200_png_context_destroy.restype = None
     _lib = L
     return L
 
@@ -862,3 +884,59 @@ class Inflator:
         buf = C.create_string_buffer(max(n, 1))
         got = self.ctx._lib.pngb200_inflator_pull_all(self.handle, buf, n)
         return buf.raw[:got]
+
+
+class PngContext:
+    """PNG.Context (online decoding) on the GPU: push each IDAT payload as it arrives; the storage is a valid partial
+    image after every push.  `pixels`: None for host storage owned by this object (storage() returns bytes), or a
+    device buffer on the context's GPU as (address, length) (storage() returns the address)."""
+
+    def __init__(self, ctx: Context, width: int, height: int, volume: int, depth: int, interlaced: bool = False,
+                 standard: int = 0, pixels=None):
+        self.ctx = ctx
+        self._size = storage_size(width, height, volume)
+        if pixels is None:
+            self._host = C.create_string_buffer(max(self._size, 1))
+            addr, cap, mem = C.addressof(self._host), self._size, MEM_HOST
+        else:
+            self._host = None
+            (addr, cap), mem = pixels, MEM_DEVICE
+        d = PngContextDesc(pixels=addr, pixels_cap=cap, width=width, height=height, volume=volume, depth=depth,
+                           interlaced=int(interlaced), standard=standard, memspace=mem)
+        self.handle = ctx._lib.pngb200_png_context_create(ctx.handle, C.byref(d))
+        if not self.handle:
+            raise PNGB200Error(ERR_BAD_ARGUMENT, ctx._lib.pngb200_last_error(ctx.handle).decode())
+        self._addr = addr
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.ctx._lib.pngb200_png_context_destroy(self.handle)
+            self.handle = None
+
+    __del__ = close
+
+    def push(self, data: bytes, overdraw: bool = False) -> None:
+        """push(data:overdraw:); raises PNGB200Error (with .payload for inflate errors) as the reference throws"""
+        st = self.ctx._lib.pngb200_png_context_push(self.handle, bytes(data), len(data), int(overdraw))
+        if st < 0:
+            s, a, b = C.c_int(), C.c_uint32(), C.c_uint32()
+            self.ctx._lib.pngb200_png_context_error(self.handle, C.byref(s), C.byref(a), C.byref(b))
+            e = PNGB200Error(st, self.ctx._lib.pngb200_last_error(self.ctx.handle).decode())
+            e.payload = (a.value, b.value) if s.value == st else (0, 0)
+            raise e
+
+    def end(self) -> None:
+        """push(ancillary:) with IEND: raises PNGB200Error(ERR_PNG_INCOMPLETE_DATASTREAM) unless the stream is complete"""
+        st = self.ctx._lib.pngb200_png_context_end(self.handle)
+        if st < 0:
+            raise PNGB200Error(st, "incomplete image data stream")
+
+    def progress(self):
+        """(next pass or 7, next row, filtered bytes consumed, stream complete, first row, end row the last push wrote)"""
+        out = (C.c_uint64 * 6)()
+        self.ctx.check(self.ctx._lib.pngb200_png_context_progress(self.handle, out))
+        return tuple(out)
+
+    def storage(self):
+        """host storage: its bytes; device storage: its address"""
+        return C.string_at(self._addr, self._size) if self._host is not None else self._addr

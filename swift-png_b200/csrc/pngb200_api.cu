@@ -1985,6 +1985,257 @@ void pngb200_inflator_error(const pngb200_inflator* z, int* status, uint32_t* a,
     if (b) *b = z->err_b;
 }
 
+// ---------------- online decoding: PNG.Context ----------------
+// The inflator handle decodes; its output is its window and is re-decoded from the last block boundary on every push, so
+// the rows it makes available are copied into `d_filt`, the context's copy of the filtered stream, and reconstructed
+// there.  Storage is written by context_assign_kernel, in `d_img` for host storage (the rows a push wrote are then
+// copied back) or straight into the caller's device storage.
+struct pngb200_png_context {
+    pngb200_ctx*      ctx = nullptr;
+    pngb200_inflator* z = nullptr;
+    uint32_t          w = 0, h = 0;
+    uint32_t          volume = 0, depth = 0;
+    bool              interlaced = false;
+    int               memspace = 0;
+    uint8_t*          pixels = nullptr;   // the caller's storage
+    uint64_t          storage = 0;        // its bytes
+    uint64_t          fsize = 0;          // filtered bytes of the image
+    DevBuf            d_img, d_filt, d_jobs;
+    PinBuf            h_jobs;
+    uint64_t          copied = 0;         // bytes of d_filt filled
+    uint64_t          drained = 0;        // bytes the decoder has pulled once every row was assigned
+    int               pass = 0;           // next pass, 7 once every row is assigned (PNG.Decoder.pass)
+    uint64_t          row = 0;            // next row of that pass
+    bool              terminal = false;   // the stream is complete (Decoder.continue == nil)
+    int               status = PNGB200_OK;
+    uint32_t          err_a = 0, err_b = 0;
+    uint64_t          band[2] = {0, 0};   // storage rows the last push wrote
+};
+
+pngb200_png_context* pngb200_png_context_create(pngb200_ctx* ctx, const pngb200_png_context_desc* d)
+{
+    if (!ctx || !d) {
+        set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_context_create: null argument");
+        return nullptr;
+    }
+    Geometry g;
+    const bool whole = d->depth >= 8 && d->volume % 8 == 0;   // g.fast admits volumes that are not whole bytes
+    if (!geometry(d->width, d->height, d->volume, d->depth, d->interlaced, &g) || !(g.passes || (g.fast && whole))) {
+        set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_context_create: bad geometry %ux%u volume %d depth %d", d->width,
+                  d->height, d->volume, d->depth);
+        return nullptr;
+    }
+    if (d->standard > 1 || (d->memspace != PNGB200_MEM_HOST && d->memspace != PNGB200_MEM_DEVICE) || !d->pixels ||
+        d->pixels_cap < g.storage) {
+        set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_context_create: bad standard, memspace or storage (%zu bytes, need %llu)",
+                  d->pixels_cap, (unsigned long long)g.storage);
+        return nullptr;
+    }
+    DeviceGuard guard(ctx->device);
+    pngb200_png_context* c = new pngb200_png_context();
+    c->ctx = ctx;
+    c->w = d->width;
+    c->h = d->height;
+    c->volume = d->volume;
+    c->depth = d->depth;
+    c->interlaced = d->interlaced != 0;
+    c->memspace = d->memspace;
+    c->pixels = (uint8_t*)d->pixels;
+    c->storage = g.storage;
+    c->fsize = g.filtered;
+    c->drained = g.filtered;
+    c->z = pngb200_inflator_create(ctx, d->standard ? PNGB200_FORMAT_IOS : PNGB200_FORMAT_ZLIB);
+    // PNG.Image(..., uninitialized: false): storage starts out zeroed
+    cudaError_t e = c->d_filt.reserve(c->fsize + 16);
+    if (e == cudaSuccess && c->memspace == PNGB200_MEM_HOST) {
+        memset(c->pixels, 0, c->storage);
+        e = c->d_img.reserve(c->storage);
+        if (e == cudaSuccess) e = cudaMemsetAsync(c->d_img.p, 0, c->storage, ctx->stream);
+    } else if (e == cudaSuccess) {
+        e = cudaMemsetAsync(c->pixels, 0, c->storage, ctx->stream);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) {
+        set_error(ctx, PNGB200_ERR_CUDA, "png_context_create: %s", cudaGetErrorString(e));
+        pngb200_png_context_destroy(c);
+        return nullptr;
+    }
+    return c;
+}
+
+void pngb200_png_context_destroy(pngb200_png_context* c)
+{
+    if (!c) return;
+    pngb200_inflator_destroy(c->z);   // synchronises the stream
+    delete c;
+}
+
+// Filtered bytes the reference's inflator makes available for the input pushed so far, beyond the inflator handle's
+// `produced`: the handle leaves a stored block whose payload has not fully arrived for the next push, while
+// LZ77.Inflator releases its payload byte by byte (Stream.readBlock(upTo:), Stream.swift:384-399).  Sets *src to
+// where those bytes start in the input.
+static uint64_t stored_in_flight(const pngb200_inflator* z, uint64_t* src)
+{
+    if (z->terminal || z->status < 0 || z->phase != 1 || z->produced != z->resume_out) return 0;
+    const std::vector<uint8_t>& in = z->input;
+    const uint64_t b = z->resume_bit, bits = 8 * (uint64_t)in.size();
+    if (b + 3 > bits || ((in[(b + 1) >> 3] >> ((b + 1) & 7)) & 1) || ((in[(b + 2) >> 3] >> ((b + 2) & 7)) & 1)) return 0;
+    const uint64_t boundary = (b + 3 + 7) & ~(uint64_t)7;
+    if (boundary + 32 > bits) return 0;
+    const uint64_t len = in[boundary >> 3] | ((uint64_t)in[(boundary >> 3) + 1] << 8);
+    *src = (boundary >> 3) + 4;
+    return std::min<uint64_t>(len, in.size() - *src);
+}
+
+int pngb200_png_context_push(pngb200_png_context* c, const uint8_t* data, size_t n, int overdraw)
+{
+    if (!c || (!data && n)) return PNGB200_ERR_BAD_ARGUMENT;
+    pngb200_ctx* ctx = c->ctx;
+    if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_context_push: a decode batch is pending");
+    c->band[0] = c->band[1] = 0;
+    if (c->status < 0) return c->status;
+    if (c->terminal) return PNGB200_ERR_PNG_EXTRANEOUS_COMPRESSED_DATA;   // PNG.Decoder.swift:51-55
+    DeviceGuard guard(ctx->device);
+    const int rc = pngb200_inflator_push(c->z, data, n);
+    if (rc < 0) {   // no row of this push is assigned
+        int s;
+        pngb200_inflator_error(c->z, &s, &c->err_a, &c->err_b);
+        if (s != rc) c->err_a = c->err_b = 0;   // not a stream error (CUDA, capacity): no payload
+        return c->status = rc;
+    }
+    c->terminal = rc == PNGB200_OK;
+    uint64_t src = 0;
+    const uint64_t decoded = c->z->produced;
+    const uint64_t avail = decoded + stored_in_flight(c->z, &src);
+    const uint64_t fill = std::min(avail, c->fsize);
+    uint8_t* filt = c->d_filt.as<uint8_t>();
+    if (fill > c->copied) {
+        const uint64_t a = std::min(fill, decoded);
+        if (a > c->copied)
+            CU(cudaMemcpyAsync(filt + c->copied, c->z->d_out.as<uint8_t>() + c->copied, a - c->copied,
+                               cudaMemcpyDeviceToDevice, ctx->stream));
+        const uint64_t b = std::max(c->copied, decoded);
+        if (fill > b)
+            CU(cudaMemcpyAsync(filt + b, c->z->d_in.as<uint8_t>() + src + (b - decoded), fill - b, cudaMemcpyDeviceToDevice,
+                               ctx->stream));
+        c->copied = fill;
+    }
+    // PNG.Decoder.push's row loop (PNG.Decoder.swift:58-140): every complete scanline, in pass order, from where the last
+    // push stopped.  The first row a pass resumes at is reconstructed again from the row above it, whose filter byte
+    // becomes None: that row already holds its pixels, so it comes out unchanged and serves as the row above.
+    struct Range { int z; uint64_t r0, r1; };
+    std::vector<Range>   ranges;
+    std::vector<PassJob> jobs;
+    const uint32_t bpp = (c->volume + 7) >> 3;
+    int z = c->pass;
+    for (; z < 7; ++z) {
+        const Pass ps = stream_pass(z, c->w, c->h, c->volume, c->interlaced);
+        if (ps.height == 0) continue;
+        const uint64_t off  = stream_pass_offset(z, c->w, c->h, c->volume, c->interlaced);
+        const uint64_t r0   = z == c->pass ? c->row : 0;
+        const uint64_t have = c->copied > off ? (c->copied - off) / (ps.pitch + 1) : 0;
+        const uint64_t r1   = std::min<uint64_t>(have, ps.height);
+        if (r1 > r0) {
+            const uint64_t start = r0 ? r0 - 1 : 0;
+            uint8_t* first = filt + off + start * (ps.pitch + 1);
+            if (r0) CU(cudaMemsetAsync(first, 0, 1, ctx->stream));
+            jobs.push_back({first, nullptr, (r1 - start) * (ps.pitch + 1), 0, (uint32_t)(r1 - start), (uint32_t)ps.pitch, bpp});
+            ranges.push_back({z, r0, r1});
+        }
+        if (r1 < ps.height) {
+            c->pass = z;
+            c->row = r1;
+            break;
+        }
+    }
+    if (z == 7) {
+        c->pass = 7;
+        c->row = 0;
+    }
+    uint8_t* img = c->memspace == PNGB200_MEM_HOST ? c->d_img.as<uint8_t>() : c->pixels;
+    if (!jobs.empty()) {
+        std::vector<uint32_t> band_base, level_start;
+        const uint64_t bands = plan_bands(jobs, band_base, level_start);
+        Tables t(c->h_jobs, c->d_jobs);
+        const size_t off_jobs = t.host(jobs.data(), sizeof(PassJob) * jobs.size());
+        const size_t off_bb = t.host(band_base.data(), sizeof(uint32_t) * band_base.size());
+        const size_t off_ls = t.host(level_start.data(), sizeof(uint32_t) * level_start.size());
+        const size_t off_pr = t.device(sizeof(uint32_t) * (bands + 1), true);   // per-band progress, then the ticket
+        if (int e = t.upload(ctx)) return e;
+        WaveParams p;
+        p.jobs = t.dev<PassJob>(off_jobs);
+        p.band_base = t.dev<uint32_t>(off_bb);
+        p.progress = t.dev<uint32_t>(off_pr);
+        p.ticket = p.progress + bands;
+        p.hist = nullptr;
+        p.njobs = (uint32_t)jobs.size();
+        p.total_bands = (uint32_t)bands;
+        p.level_start = t.dev<uint32_t>(off_ls);
+        p.levels = level_start.empty() ? 0u : (uint32_t)level_start.size() - 1;
+        const unsigned grid = (unsigned)std::min<uint64_t>((bands + WAVE_WARPS - 1) / WAVE_WARPS, (uint64_t)ctx->sm_count * 8);
+        unfilter_pass_kernel<<<grid, WAVE_WARPS * 32, WAVE_SMEM, ctx->stream>>>(p);
+        ctx->launches++;
+        CU(cudaGetLastError());
+        // one launch per pass, in pass order: a later pass paints over an earlier one
+        c->band[0] = c->h;
+        for (const Range& r : ranges) {
+            AssignJob j;
+            uint64_t  y0, y1;
+            const uint32_t ctas = plan_assign(r.z, r.r0, r.r1, filt, img, c->w, c->h, c->volume, c->depth, c->interlaced,
+                                              overdraw != 0, (unsigned)ctx->sm_count * 16, &j, &y0, &y1);
+            context_assign_kernel<<<ctas, ASSIGN_THREADS, 0, ctx->stream>>>(j);
+            ctx->launches++;
+            CU(cudaGetLastError());
+            c->band[0] = std::min(c->band[0], y0);
+            c->band[1] = std::max(c->band[1], y1);
+        }
+        if (c->memspace == PNGB200_MEM_HOST) {
+            const uint64_t pitch = (uint64_t)c->w * bpp;
+            CU(cudaMemcpyAsync(c->pixels + c->band[0] * pitch, img + c->band[0] * pitch, (c->band[1] - c->band[0]) * pitch,
+                               cudaMemcpyDeviceToHost, ctx->stream));
+        }
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+    // every row is assigned: any filtered byte beyond them is an error, in this push and in any later one
+    // (PNG.Decoder.swift:142-147; the bytes are drained, as inflator.pull() drains them)
+    if (c->pass == 7 && avail > c->drained) {
+        c->drained = avail;
+        return PNGB200_ERR_PNG_EXTRANEOUS_IMAGE_DATA;
+    }
+    return PNGB200_OK;
+}
+
+int pngb200_png_context_end(pngb200_png_context* c)
+{
+    if (!c) return PNGB200_ERR_BAD_ARGUMENT;
+    return c->terminal ? PNGB200_OK : PNGB200_ERR_PNG_INCOMPLETE_DATASTREAM;   // PNG.Context.swift:134-141
+}
+
+int pngb200_png_context_progress(const pngb200_png_context* c, uint64_t out[6])
+{
+    if (!c || !out) return PNGB200_ERR_BAD_ARGUMENT;
+    out[0] = (uint64_t)c->pass;
+    out[1] = c->row;
+    if (c->pass == 7) {
+        out[2] = c->drained;
+    } else {
+        const Pass ps = stream_pass(c->pass, c->w, c->h, c->volume, c->interlaced);
+        out[2] = stream_pass_offset(c->pass, c->w, c->h, c->volume, c->interlaced) + c->row * (ps.pitch + 1);
+    }
+    out[3] = c->terminal ? 1 : 0;
+    out[4] = c->band[0];
+    out[5] = c->band[1];
+    return PNGB200_OK;
+}
+
+void pngb200_png_context_error(const pngb200_png_context* c, int* status, uint32_t* a, uint32_t* b)
+{
+    if (!c) return;
+    if (status) *status = c->status;
+    if (a) *a = c->err_a;
+    if (b) *b = c->err_b;
+}
+
 }  // extern "C"
 
 #include "png_file.cuh"

@@ -23,6 +23,10 @@
 //   filtered stream; unfilter_interleave_kernel then writes PNG.Image.storage from the pass rows.
 //
 // unfilter_generic_kernel: the same formats when the filtered stream is short; one CTA per image.
+//
+// context_assign_kernel (online decoding, pngb200_png_context): PNG.Image.assign of a range of one pass's rows, which
+// unfilter_pass_kernel reconstructed in the context's copy of the filtered stream, and PNG.Image.overdraw of each row
+// (PNG.Image.swift:133-183).
 #pragma once
 
 #include <algorithm>
@@ -545,6 +549,18 @@ __global__ void __launch_bounds__(128) unfilter_generic_kernel(const GenericJob*
 // ---- the pass path's second kernel: PNG.Image.assign from the rows unfilter_pass_kernel reconstructed in place ----
 constexpr int INTERLEAVE_THREADS = 256;   // one aligned 16-byte chunk of storage per thread and block
 
+// Byte c of pixel i of a reconstructed pass row, as PNG.Image.assign stores it: a 1/2/4-bit sample MSB-first, one byte
+// per pixel (8 >> lper samples a byte), otherwise byte c of the pixel's bpp bytes.
+__device__ __forceinline__ uint32_t pass_sample(const uint8_t* line, uint64_t i, uint32_t c, uint32_t bpp, uint32_t depth,
+                                                uint32_t lper)
+{
+    if (depth < 8) {
+        const uint32_t sh = ((~(uint32_t)i) & ((1u << lper) - 1)) * depth;
+        return (line[i >> lper] >> sh) & ((1u << depth) - 1);
+    }
+    return line[i * bpp + c];
+}
+
 // Every byte of an image's storage, in output order: a block writes 4 KiB that are contiguous in memory, a thread one
 // aligned 16-byte chunk of it with a single store, so that every store fills whole 32-byte sectors.  A pixel takes its
 // sample from its pass row (Adam7 origin and step per c_adam7; a 1/2/4-bit sample MSB-first, one byte per pixel), or
@@ -599,15 +615,7 @@ __global__ void __launch_bounds__(INTERLEAVE_THREADS) unfilter_interleave_kernel
             const uint64_t r  = y >> ey;   // (y - origin) >> step: the origin's bits sit below the step
             const uint64_t i  = x >> ex;
             uint32_t       v  = 0;
-            if (r < s_rows[z]) {
-                const uint8_t* line = s_line[z] + r * s_stride[z];
-                if (job.depth < 8) {   // 1, 2 or 4 bits: 8 >> lper samples a byte
-                    const uint32_t sh = ((~(uint32_t)i) & ((1u << lper) - 1)) * job.depth;
-                    v = (line[i >> lper] >> sh) & ((1u << job.depth) - 1);
-                } else {
-                    v = line[i * bpp + c];
-                }
-            }
+            if (r < s_rows[z]) v = pass_sample(s_line[z] + r * s_stride[z], i, c, bpp, job.depth, lper);
             const uint32_t slot = (uint32_t)(at - (uint64_t)first), sv = v << (8 * (slot & 3));
             w0 |= slot < 4 ? sv : 0u;   // selects, not w[slot >> 2]: a dynamically indexed array goes to local memory
             w1 |= slot >> 2 == 1 ? sv : 0u;
@@ -685,6 +693,110 @@ inline void plan_passes(InterleaveJob image, std::vector<PassJob>& passes, std::
     images.push_back(image);
     const uint64_t chunks = (15 + (uint64_t)image.width * image.height * image.bpp + 15) / 16;   // any misalignment of the pixels
     blocks += (chunks + INTERLEAVE_THREADS - 1) / INTERLEAVE_THREADS;
+}
+
+// ---- online decoding (pngb200_png_context): PNG.Image.assign, and PNG.Image.overdraw, of a range of one pass's rows ----
+constexpr int ASSIGN_THREADS = 256;
+
+// Rows [r0, r1) of pass (bx, by, ex, ey), reconstructed in the context's copy of the filtered stream, for
+// context_assign_kernel.  `tiles` CTAs share each row.
+struct AssignJob {
+    const uint8_t* line;           // pixel bytes of row r0 (behind its filter byte)
+    uint8_t*       pixels;         // PNG.Image.storage
+    uint64_t       stride;         // pitch + 1
+    uint64_t       pass_width;     // pixels per row of the pass
+    uint32_t       width, height;  // of the image
+    uint32_t       r0, r1;
+    uint32_t       bx, by, ex, ey;
+    uint32_t       tiles;
+    uint8_t        bpp, depth, overdraw;
+};
+
+// The brush PNG.Context.push(data:overdraw:) paints row Y of a pass with (PNG.Context.swift:89-95): the stride, halved
+// across when the pass does not start at x = 0 and halved down when Y is not a multiple of 8.  Width * height <= 1 paints
+// nothing (PNG.Image.swift:133-139).
+__host__ __device__ __forceinline__ void overdraw_brush(uint32_t bx, uint32_t ex, uint32_t ey, uint64_t Y, uint32_t* bw,
+                                                        uint32_t* bh)
+{
+    *bw = (1u << ex) >> (bx != 0 ? 1 : 0);
+    *bh = (1u << ey) >> ((Y & 7) != 0 ? 1 : 0);
+}
+
+// Every row of the job is assigned (PNG.Image.assign, PNG.Image.swift:186-285) and, with `overdraw`, painted with its
+// brush (PNG.Image.overdraw, PNG.Image.swift:133-183): for x = bx, bx + brush.x, ... < width, pixels x ... x + brush.x - 1
+// of rows Y ... Y + brush.y - 1, clipped at the image's edge, become pixel (x, Y).  A thread writes one target pixel.  Its
+// source (x, Y) is a pixel of the row itself, taken from the scanline, or a pixel an earlier pass assigned, read from
+// storage: the rectangles of one pass's rows are disjoint and a source is only ever written with its own value, which
+// is skipped, so no thread writes what another one reads.  Passes must still be launched in order: a later pass paints
+// over an earlier one.
+__global__ void __launch_bounds__(ASSIGN_THREADS) context_assign_kernel(AssignJob j)
+{
+    const uint32_t lper  = j.depth == 1 ? 3 : j.depth == 2 ? 2 : 1;
+    const uint32_t sx    = 1u << j.ex;
+    const uint32_t tiles = (j.r1 - j.r0) * j.tiles;   // plan_assign keeps the product below 2^32
+    for (uint32_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+        const uint32_t r    = j.r0 + t / j.tiles;
+        const uint32_t tile = t % j.tiles;
+        const uint64_t Y    = j.by + ((uint64_t)r << j.ey);
+        const uint8_t* line = j.line + (uint64_t)(r - j.r0) * j.stride;
+        uint32_t bw, bh;
+        overdraw_brush(j.bx, j.ex, j.ey, Y, &bw, &bh);
+        const bool     paint = j.overdraw && bw * bh > 1;
+        const uint32_t lbw   = j.ex - (j.bx != 0 ? 1 : 0);   // log2 of the brush width
+        const uint32_t rows  = paint ? (uint32_t)min((uint64_t)bh, j.height - Y) : 1;
+        const uint64_t cols  = paint ? j.width - j.bx : j.pass_width;
+        for (uint32_t dy = 0; dy < rows; ++dy) {
+            uint8_t* out = j.pixels + (Y + dy) * j.width * j.bpp;
+            for (uint64_t q = (uint64_t)tile * ASSIGN_THREADS + threadIdx.x; q < cols; q += (uint64_t)j.tiles * ASSIGN_THREADS) {
+                const uint64_t x   = paint ? j.bx + q : j.bx + (q << j.ex);     // target column
+                const uint64_t xs  = paint ? j.bx + (q >> lbw << lbw) : x;      // source column, on row Y
+                const bool     own = ((xs - j.bx) & (sx - 1)) == 0;             // the source is a pixel of this row
+                if (!own && dy == 0 && x == xs) continue;
+                uint8_t* dst = out + x * j.bpp;
+                if (own) {
+                    const uint64_t i = (xs - j.bx) >> j.ex;
+                    for (uint32_t c = 0; c < j.bpp; ++c) dst[c] = (uint8_t)pass_sample(line, i, c, j.bpp, j.depth, lper);
+                } else {
+                    const uint8_t* src = j.pixels + (Y * j.width + xs) * j.bpp;
+                    for (uint32_t c = 0; c < j.bpp; ++c) dst[c] = src[c];
+                }
+            }
+        }
+    }
+}
+
+// The launch for rows [r0, r1) of pass z of an image whose filtered stream is at `filtered`, and the storage rows it
+// writes, [*y0, *y1).  Returns the number of CTAs.
+inline uint32_t plan_assign(int z, uint64_t r0, uint64_t r1, const uint8_t* filtered, uint8_t* pixels, uint32_t w, uint32_t h,
+                            uint32_t volume, uint32_t depth, bool interlaced, bool overdraw, unsigned max_ctas,
+                            AssignJob* job, uint64_t* y0, uint64_t* y1)
+{
+    const Pass     ps  = stream_pass(z, w, h, volume, interlaced);
+    const uint64_t off = stream_pass_offset(z, w, h, volume, interlaced);
+    AssignJob& j = *job;
+    j.line = filtered + off + r0 * (ps.pitch + 1) + 1;
+    j.pixels = pixels;
+    j.stride = ps.pitch + 1;
+    j.pass_width = ps.width;
+    j.width = w;
+    j.height = h;
+    j.r0 = (uint32_t)r0;
+    j.r1 = (uint32_t)r1;
+    j.bx = ps.bx; j.by = ps.by; j.ex = ps.ex; j.ey = ps.ey;
+    j.bpp = (uint8_t)((volume + 7) >> 3);
+    j.depth = (uint8_t)depth;
+    j.overdraw = overdraw;
+    // a brush is at most 8 x 8 pixels, so a row never covers more than 8 image rows
+    const uint64_t most = overdraw ? std::min<uint64_t>(8, h) * (w - ps.bx) : ps.width;
+    const uint64_t rows = r1 - r0;
+    j.tiles = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((most + ASSIGN_THREADS - 1) / ASSIGN_THREADS,
+                                                                 std::max<uint64_t>(1, max_ctas / rows)));
+    const uint64_t last = ps.by + ((r1 - 1) << ps.ey);
+    uint32_t bw, bh;
+    overdraw_brush(ps.bx, ps.ex, ps.ey, last, &bw, &bh);
+    *y0 = ps.by + (r0 << ps.ey);
+    *y1 = overdraw && bw * bh > 1 ? std::min<uint64_t>(last + bh, h) : last + 1;
+    return (uint32_t)std::min<uint64_t>(rows * j.tiles, max_ctas);
 }
 
 }  // namespace pngb200
