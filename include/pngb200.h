@@ -410,7 +410,10 @@ int    pngb200_png_encode_files(pngb200_ctx* ctx, pngb200_png_encode_desc* image
 size_t pngb200_filtered_size(uint32_t width, uint32_t height, int volume, int interlaced);
 size_t pngb200_storage_size(uint32_t width, uint32_t height, int volume);
 
-/* ---- streaming handles (LZ77.Inflator value-type semantics, layered on the batch path) ---- */
+/* ---- streaming handles (LZ77.Inflator value-type semantics, layered on the batch path) ----
+ * Each push decodes only input no earlier push decoded: it resumes where the last one stopped, at a block header or,
+ * inside a fixed or dynamic block, at the last complete symbol (whose block header is parsed again).  A stored block
+ * is released once all of it has arrived. */
 typedef struct pngb200_inflator pngb200_inflator;
 /* LZ77.Inflator.init(format:) / Gzip.Inflator.init(), LZ77.Inflator.swift:18-23 */
 pngb200_inflator* pngb200_inflator_create(pngb200_ctx* ctx, int format);
@@ -424,6 +427,9 @@ int    pngb200_inflator_pull(pngb200_inflator* z, uint8_t* dst, size_t count);
 size_t pngb200_inflator_pull_all(pngb200_inflator* z, uint8_t* dst, size_t cap);
 size_t pngb200_inflator_available(const pngb200_inflator* z);
 void   pngb200_inflator_error(const pngb200_inflator* z, int* status, uint32_t* a, uint32_t* b);
+/* Work the device has done for this handle since it was created: out[0] input bits decoded (a bit decoded twice counts
+ * twice), out[1] output bytes written (likewise), out[2] of those written by the one-warp serial decoder. */
+int    pngb200_inflator_stats(const pngb200_inflator* z, uint64_t out[3]);
 
 /* ---- online decoding: PNG.Context (Sources/PNG/Decoding/PNG.Context.swift) ----------------------------------------
  * A caller pushes each IDAT chunk as it arrives; after every push the storage is a valid partial image.  Restates

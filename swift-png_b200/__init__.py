@@ -300,6 +300,9 @@ def lib():
     L.pngb200_inflator_error.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_uint32),
                                          C.POINTER(C.c_uint32)]
     L.pngb200_inflator_error.restype = None
+    if os.environ.get("PNGB200_LIB") is None or hasattr(L, "pngb200_inflator_stats"):   # (older builds lack it)
+        L.pngb200_inflator_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.pngb200_inflator_stats.restype = C.c_int
     if os.environ.get("PNGB200_LIB") is None or hasattr(L, "pngb200_png_context_create"):   # (older builds lack it)
         L.pngb200_png_context_create.argtypes = [C.c_void_p, C.POINTER(PngContextDesc)]
         L.pngb200_png_context_create.restype = C.c_void_p
@@ -884,6 +887,15 @@ class Inflator:
         buf = C.create_string_buffer(max(n, 1))
         got = self.ctx._lib.pngb200_inflator_pull_all(self.handle, buf, n)
         return buf.raw[:got]
+
+    def stats(self) -> dict:
+        """Work the device has done for this handle: input bits decoded and output bytes written (a bit or byte
+        decoded twice counts twice), and the bytes of those the one-warp serial decoder wrote."""
+        out = (C.c_uint64 * 3)()
+        st = self.ctx._lib.pngb200_inflator_stats(self.handle, out)
+        if st != OK:
+            raise PNGB200Error(st, "inflator_stats")
+        return {"bits": out[0], "bytes": out[1], "serial_bytes": out[2]}
 
 
 class PngContext:

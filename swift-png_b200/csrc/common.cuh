@@ -14,16 +14,31 @@
 
 namespace pngb200 {
 
+// Where a streaming decode stopped inside a fixed or dynamic block, and the work one launch did.  Only the streaming
+// handle passes one (StreamJob.resume); the kernel reads the position when the job starts in phase 3 and writes it
+// when it stops inside a Huffman block for want of input (StreamResult.phase 3).
+struct ResumePoint {
+    uint64_t header_bit;   // the block's header
+    uint64_t symbol_bit;   // its next undecoded symbol
+    uint64_t out;          // output size at symbol_bit
+    uint32_t final;        // the block's BFINAL
+    uint32_t pad_;
+    // the launch's work, set by the kernel: input bits decoded (a bit decoded twice counts twice), output bytes
+    // written, and how many of those the one-warp serial decoder wrote
+    uint64_t bits, bytes, serial_bytes;
+};
+
 // One DEFLATE stream to inflate (device-resident record).
 struct StreamJob {
     const uint8_t* src;
     uint64_t       src_len;
     uint8_t*       dst;
     uint64_t       dst_cap;
-    uint64_t       start_bit;   // resume point (bit offset of a block header), 0 = from the top
+    uint64_t       start_bit;   // resume point (bit offset of a block header, or of a symbol in phase 3), 0 = the top
     uint64_t       start_out;   // bytes already produced before start_bit
     int32_t        format;      // pngb200_format
-    int32_t        phase;       // where to resume: 0 stream header, 1 block header, 2 trailer
+    int32_t        phase;       // where to resume: 0 stream header, 1 block header, 2 trailer, 3 inside the Huffman
+                                // block whose header is at resume->header_bit (its header is parsed again)
     // segments of a stream that several CTAs decode side by side (inflate_wave_kernel only):
     uint64_t       stop_bit;    // 0 = to the end of the stream; else stop at the first block boundary >= stop_bit
     uint32_t       symbolic;    // 1: dst is uint16_t[dst_cap]; a byte copied from in front of the segment becomes
@@ -34,6 +49,9 @@ struct StreamJob {
     // stream is inflated (the image's pixel buffer, written by unfilter afterwards), or null
     uint8_t*       scratch;
     uint64_t       scratch_cap;
+    // the streaming handle's resume record (serial and ring kernels only), or null: then a decode that runs out of
+    // input inside a block resumes at the block's header
+    ResumePoint*   resume;
 };
 
 struct StreamResult {

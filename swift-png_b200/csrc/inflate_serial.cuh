@@ -281,17 +281,24 @@ __device__ int read_trailer(BitReader& br, int format, StreamResult* r)
     return PNGB200_OK;
 }
 
-// The whole serial decode of one stream by one warp, from (start_bit, start_out, phase).
+// The whole serial decode of one stream by one warp, from (start_bit, start_out, phase).  In phase 3, start_bit is a
+// symbol inside the Huffman block whose header is at `header_bit`: the header is parsed again and decoding goes on at
+// start_bit.  With a resume record (job.resume), input that ends inside a Huffman block leaves the resume point at
+// the last complete symbol (phase 3), and the launch's work is added to the record's counters.
 // `r` must have been zeroed (status 0) by the caller.
 __device__ void serial_inflate(SerialShared& sh, const StreamJob& job, StreamResult* r, uint64_t start_bit,
-                               uint64_t start_out, uint32_t phase, uint32_t blocks)
+                               uint64_t start_out, uint32_t phase, uint32_t blocks, uint64_t header_bit = 0)
 {
     const unsigned lane = lane_id();
     BitReader      br;
-    br.init(job.src, job.src_len, start_bit);
+    br.init(job.src, job.src_len, phase == 3 ? header_bit : start_bit);
     uint64_t out = start_out;
     int      st  = PNGB200_OK;
     uint64_t resume_bit = start_bit, resume_out = start_out;
+    uint64_t reparsed = 0;          // header bits parsed again to resume inside a block
+    bool     inside = phase == 3;   // the next header is that of the block to resume in
+    uint64_t hdr_bit = header_bit;  // the current block's header and BFINAL (for a phase-3 resume point)
+    int      final = 0;
 
     if (phase == 0) {
         st = read_stream_header(br, job.format, r);
@@ -302,13 +309,19 @@ __device__ void serial_inflate(SerialShared& sh, const StreamJob& job, StreamRes
     }
     uint8_t* dst = job.dst;
     if (st == PNGB200_OK && phase == 2) st = read_trailer(br, job.format, r);
-    while (st == PNGB200_OK && phase == 1) {
-        int      type, final;
+    while (st == PNGB200_OK && (phase == 1 || phase == 3)) {
+        int      type;
         uint32_t stored = 0;
         int nlit = 0, ndist = 0;
+        hdr_bit = br.at();
         st = parse_block_header(br, &sh, r, (int)lane, &type, &final, &stored, &nlit, &ndist);
         if (st == PNGB200_OK && type != 0) st = build_block_tables(&sh, r, nlit, ndist, (int)lane, 32);
         if (st != PNGB200_OK) break;
+        if (inside) {
+            reparsed = br.at() - hdr_bit;
+            br.seek(br.lead_bits + start_bit);
+            inside = false;
+        }
         if (type == 0) {
             // Stream.readBlock(upTo:), Stream.swift:384-399 -- byte-aligned copy
             if (!br.have(8 * (uint64_t)stored)) { st = PNGB200_NEED_MORE_INPUT; break; }
@@ -320,7 +333,9 @@ __device__ void serial_inflate(SerialShared& sh, const StreamJob& job, StreamRes
             __syncwarp();
         } else {
             // Stream.readBlock(with:), Stream.swift:266-381
+            uint64_t sym_bit = br.at();   // the symbol being decoded starts here
             for (;;) {
+                sym_bit = br.at();
                 br.refill();
                 uint32_t e   = lookup<LIT_ROOT>(sh.lit, br.peek());
                 uint32_t len = e_len(e), kind = e_kind(e);
@@ -365,11 +380,19 @@ __device__ void serial_inflate(SerialShared& sh, const StreamJob& job, StreamRes
                     break;
                 }
             }
+            if (st == PNGB200_NEED_MORE_INPUT && job.resume) {
+                // stop at the last complete symbol: `out` holds exactly the bytes of the symbols before sym_bit
+                resume_bit = sym_bit;
+                resume_out = out;
+                phase      = 3;
+                br.seek(br.lead_bits + sym_bit);
+            }
             if (st != PNGB200_OK) break;
         }
         ++blocks;
         resume_bit = br.at();
         resume_out = out;
+        phase = 1;
         if (final) {
             phase = 2;
             st = read_trailer(br, job.format, r);
@@ -384,6 +407,14 @@ __device__ void serial_inflate(SerialShared& sh, const StreamJob& job, StreamRes
         r->resume_bit    = resume_bit;
         r->resume_out    = resume_out;
         r->phase         = phase;
+        if (job.resume) {
+            if (phase == 3) *job.resume = ResumePoint{hdr_bit, resume_bit, resume_out, (uint32_t)final, 0,
+                                                      job.resume->bits, job.resume->bytes, job.resume->serial_bytes};
+            const uint64_t to = br.at() < br.size() ? br.at() : br.size();
+            job.resume->bits += reparsed + (to > start_bit ? to - start_bit : 0);
+            job.resume->bytes += out - start_out;
+            job.resume->serial_bytes += out - start_out;
+        }
     }
 }
 
@@ -394,7 +425,8 @@ __global__ void __launch_bounds__(32) inflate_serial_kernel(const StreamJob* job
     if ((int)blockIdx.x >= count) return;
     const int j = order ? (int)order[blockIdx.x] : (int)blockIdx.x;
     const StreamJob job = jobs[j];
-    serial_inflate(sh, job, results + j, job.start_bit, job.start_out, (uint32_t)job.phase, 0);
+    serial_inflate(sh, job, results + j, job.start_bit, job.start_out, (uint32_t)job.phase, 0,
+                   job.phase == 3 ? job.resume->header_bit : 0);
 }
 
 }  // namespace pngb200

@@ -515,6 +515,9 @@ struct StreamRun {
     uint32_t      blocks, phase;
     int           st;
     bool          fallback;   // the serial decoder redoes the stream from the resume point
+    // With a resume record (job.resume), thread 0 keeps the block being decoded there: its header, and the last wave
+    // checkpoint inside it (symbol_bit, out; symbol_bit = 0: none yet), where the serial decoder takes over.  The
+    // checkpoints live in the record rather than in registers, which the ring kernel has none to spare of.
 
     // job `j` of the batch: its stream header, or its trailer when the job starts there
     __device__ __forceinline__ void open(const WvParams& P, int j)
@@ -529,6 +532,11 @@ struct StreamRun {
         phase      = (uint32_t)job.phase;
         st         = PNGB200_OK;
         fallback   = false;
+        if (phase == 3) {
+            // inside a Huffman block: its header is parsed again (begin_block), then the first wave starts at start_bit
+            br.seek(br.lead_bits + job.resume->header_bit);
+            phase = 1;
+        }
         if (phase == 0) {
             st = read_stream_header(br, job.format, r);
             if (st == PNGB200_OK) {
@@ -537,6 +545,36 @@ struct StreamRun {
             }
         }
         if (st == PNGB200_OK && phase == 2) st = read_trailer(br, job.format, r);
+    }
+
+    // The header of a Huffman block, parsed at `hdr` (reader space), ends at the reader.  Every thread calls it; when the
+    // job resumes inside this block, the reader moves on to the resume symbol, and the header bits count as decoded.
+    __device__ __forceinline__ void begin_block(uint64_t hdr, int final)
+    {
+        if (!job.resume) return;
+        const bool resumed = job.phase == 3 && blocks == 0;
+        if (threadIdx.x == 0) {
+            job.resume->header_bit = hdr - br.lead_bits;
+            job.resume->final = (uint32_t)final;
+            if (resumed) job.resume->bits = br.pos - hdr;
+            else job.resume->symbol_bit = 0;
+        }
+        if (resumed) br.seek(br.lead_bits + job.start_bit);
+    }
+    // A wave of the current Huffman block ended at the reader, on a symbol boundary, with `out` bytes decoded
+    __device__ __forceinline__ void wave_done()
+    {
+        if (threadIdx.x == 0 && job.resume) {
+            job.resume->symbol_bit = br.at();
+            job.resume->out = out;
+        }
+    }
+    // The wave that starts at the reader cannot be decoded here: the serial decoder takes over.  The wave counts as
+    // decoded up to the end of the input.
+    __device__ __forceinline__ void fall_back()
+    {
+        fallback = true;
+        if (threadIdx.x == 0 && job.resume) job.resume->bits += min(br.at() + WV_BITS, br.size()) - job.start_bit;
     }
 
     // After a block: the resume point moves behind it.  True when the block loop ends there: at the end of a
@@ -594,8 +632,15 @@ struct StreamRun {
                 r->blocks = blocks;
             }
         } else if (fallback) {
+            if (t == 0 && job.resume) job.resume->bytes = out - job.start_out;
             __syncthreads();
-            if (t < 32) serial_inflate(sh.ser, job, r, resume_bit, resume_out, 1, blocks);
+            // with a resume record, from the last wave checkpoint of the block: at most one wave is decoded again
+            if (t < 32) {
+                const ResumePoint at = job.resume ? *job.resume : ResumePoint{};
+                const bool mid = at.symbol_bit != 0;
+                serial_inflate(sh.ser, job, r, mid ? at.symbol_bit : resume_bit, mid ? at.out : resume_out, mid ? 3 : 1,
+                               blocks, at.header_bit);
+            }
         } else if (t == 0) {
             if (r->status == 0) r->status = st;
             r->produced      = out;
@@ -605,6 +650,10 @@ struct StreamRun {
             r->resume_out    = resume_out;
             r->phase         = phase;
             if (adler_on) adler.check_trailer(r, job.format);
+            if (job.resume) {
+                job.resume->bits += br.at() - job.start_bit;
+                job.resume->bytes = out - job.start_out;
+            }
         }
         if (t == 0) r->stat_fallback = fallback ? 1u : 0u;
     }

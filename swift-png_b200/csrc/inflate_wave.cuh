@@ -43,7 +43,8 @@
 // sources from HBM and keep their bitmap in HBM scratch; the ring is refilled from HBM afterwards.
 // Anything irregular (invalid symbol on the chain, truncation, output overflow, distance before the
 // start of the output) is not handled here: warp 0 re-runs the block with the serial decoder
-// (inflate_serial.cuh), which owns the exact error semantics of the reference.
+// (inflate_serial.cuh), which owns the exact error semantics of the reference.  A job with a resume record (the
+// streaming handle) hands it only the rest of the block from the last wave that completed.
 //
 // CTAs are persistent: each takes streams from an atomic ticket (the host orders streams longest
 // first), so per-CTA scratch in HBM is bounded by the number of resident CTAs.
@@ -330,6 +331,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
         while (S.st == PNGB200_OK && S.phase == 1) {
             __syncthreads();
             adler.fold(sh);
+            const uint64_t hpos = br.pos;
             const WvHeader hdr = read_block_header(sh, br, r);
             S.st = hdr.status;
             if (S.st != PNGB200_OK) break;
@@ -339,6 +341,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
             if (type != 0) {
                 S.st = build_block_tables(&sh.ser, r, hdr.nlit, hdr.ndist, (int)t, WV_THREADS);
                 if (S.st != PNGB200_OK) break;
+                S.begin_block(hpos, final);
             }
             phase_tick(sh, 0);
             if (type == 0) {
@@ -556,7 +559,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                     const uint32_t np      = (uint32_t)(sh.warp_sums[WV_WARPS] >> 40);
                     // (bit 1 only: a thread already in phase E may have set bit 2 for this wave -- read after barrier (7))
                     if ((sh.anomaly & 1u) || out + total64 > dst_cap || total64 > P.bitmap_words * 32) {
-                        S.fallback = true;
+                        S.fall_back();
                         over_cap = out + total64 > dst_cap;
                         break;
                     }
@@ -691,7 +694,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                     if (sh.anomaly) {
                         // leave the bitmap clean for whoever uses it next
                         for (uint32_t k = t; k < (total + 31) / 32; k += WV_THREADS) U[k] = 0;
-                        S.fallback = true;
+                        S.fall_back();
                         break;
                     }
                     if (may_switch && sym) {
@@ -742,6 +745,7 @@ __global__ void __launch_bounds__(WV_THREADS, WV_CTAS_PER_SM) inflate_wave_kerne
                     n_deferred += deferred;
                     br.seek((wbase << 5) + sh.wpos_[last]);
                     if (term == WK_EOB || term == WK_OWN_EOB) block_done = true;
+                    else S.wave_done();
                     try_switch();
                 }
                 if (S.fallback) break;

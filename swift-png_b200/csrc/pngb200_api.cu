@@ -1841,6 +1841,8 @@ struct pngb200_inflator {
     size_t               uploaded = 0;
     uint64_t             resume_bit = 0, resume_out = 0, produced = 0, current = 0;
     uint32_t             phase = 0;
+    ResumePoint          at{};            // the block a phase-3 resume point lies in (uploaded with every launch)
+    uint64_t             work[3] = {};    // pngb200_inflator_stats
     bool                 terminal = false;
     int                  status = PNGB200_NEED_MORE_INPUT;
     uint32_t             err_a = 0, err_b = 0;
@@ -1896,22 +1898,30 @@ int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
         CU(cudaMemcpyAsync(z->d_in.as<uint8_t>() + z->uploaded, z->input.data() + z->uploaded,
                            z->input.size() - z->uploaded, cudaMemcpyHostToDevice, ctx->stream));
     z->uploaded = z->input.size();
+    // d_res and h_res hold the result, then the resume record; h_res then stages the job
+    constexpr size_t kIo = sizeof(StreamResult) + sizeof(ResumePoint);
     CU(z->d_job.reserve(sizeof(StreamJob)));
-    CU(z->d_res.reserve(sizeof(StreamResult)));
-    CU(z->h_res.reserve(sizeof(StreamResult) + sizeof(StreamJob)));
+    CU(z->d_res.reserve(kIo));
+    CU(z->h_res.reserve(kIo + sizeof(StreamJob)));
     int rc = inflator_grow_out(z, std::max<size_t>(1 << 16, z->produced + 4 * n + 1024));
     if (rc != PNGB200_OK) return rc;
     for (;;) {
-        StreamJob* job = (StreamJob*)((char*)z->h_res.p + sizeof(StreamResult));
+        StreamResult* res = z->h_res.as<StreamResult>();
+        ResumePoint*  at  = reinterpret_cast<ResumePoint*>(res + 1);
+        StreamJob*    job = reinterpret_cast<StreamJob*>(at + 1);
         *job = whole_stream_job(z->d_in.as<uint8_t>(), z->input.size(), z->d_out.as<uint8_t>(), z->d_out.cap, z->format);
         job->start_bit = z->resume_bit;
         job->start_out = z->resume_out;
         job->phase = (int32_t)z->phase;
+        job->resume = reinterpret_cast<ResumePoint*>(z->d_res.as<StreamResult>() + 1);
+        memset(res, 0, sizeof *res);
+        *at = z->at;
+        at->bits = at->bytes = at->serial_bytes = 0;
         CU(cudaMemcpyAsync(z->d_job.p, job, sizeof(StreamJob), cudaMemcpyHostToDevice, ctx->stream));
-        CU(cudaMemsetAsync(z->d_res.p, 0, sizeof(StreamResult), ctx->stream));
+        CU(cudaMemcpyAsync(z->d_res.p, res, kIo, cudaMemcpyHostToDevice, ctx->stream));
         // A push with a lot of undecoded input goes through the intra-stream parallel kernel (one CTA: ~25 x the
-        // lock-step warp); short ones, and everything irregular inside it, through the serial decoder.  Both resume
-        // at the last completed block boundary.
+        // lock-step warp); short ones, and what is left of the wave the input ends in, through the serial decoder.
+        // Both resume where the last push stopped: at a block header, or at the last complete symbol of a Huffman block.
         const uint64_t pending = z->input.size() - std::min<uint64_t>(z->input.size(), z->resume_bit >> 3);
         if (pending >= (64u << 10)) {
             rc = launch_waves(ctx, ENG_WAVE, z->d_job.as<StreamJob>(), z->d_res.as<StreamResult>(), nullptr, 1, 1, job->dst_cap, nullptr);
@@ -1921,7 +1931,7 @@ int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
             ctx->launches++;
         }
         CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(z->h_res.p, z->d_res.p, sizeof(StreamResult), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(z->h_res.p, z->d_res.p, kIo, cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
         // The stream checksum is only due when the trailer has been read: ONE pass over the output at the end of the
         // stream, not one per push (round 1 re-checksummed everything produced so far on every push).
@@ -1933,8 +1943,13 @@ int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
             CU(cudaMemcpyAsync(z->h_res.p, z->d_res.p, sizeof(StreamResult), cudaMemcpyDeviceToHost, ctx->stream));
             CU(cudaStreamSynchronize(ctx->stream));
         }
-        const StreamResult r = *z->h_res.as<StreamResult>();
-        // remember the last completed block boundary: the next run resumes there
+        const StreamResult r = *res;
+        z->at = *at;
+        z->work[0] += at->bits;
+        z->work[1] += at->bytes;
+        z->work[2] += at->serial_bytes;
+        // the next run resumes where this one stopped (after an output capacity error: where it started, or behind a
+        // block it completed)
         z->phase = r.phase;
         z->resume_bit = r.resume_bit;
         z->resume_out = r.resume_out;
@@ -1977,6 +1992,13 @@ size_t pngb200_inflator_pull_all(pngb200_inflator* z, uint8_t* dst, size_t cap)
     return n;
 }
 
+int pngb200_inflator_stats(const pngb200_inflator* z, uint64_t out[3])
+{
+    if (!z || !out) return PNGB200_ERR_BAD_ARGUMENT;
+    for (int k = 0; k < 3; ++k) out[k] = z->work[k];
+    return PNGB200_OK;
+}
+
 void pngb200_inflator_error(const pngb200_inflator* z, int* status, uint32_t* a, uint32_t* b)
 {
     if (!z) return;
@@ -1986,7 +2008,7 @@ void pngb200_inflator_error(const pngb200_inflator* z, int* status, uint32_t* a,
 }
 
 // ---------------- online decoding: PNG.Context ----------------
-// The inflator handle decodes; its output is its window and is re-decoded from the last block boundary on every push, so
+// The inflator handle decodes; each push resumes where the last one stopped, and its output is its window, so
 // the rows it makes available are copied into `d_filt`, the context's copy of the filtered stream, and reconstructed
 // there.  Storage is written by context_assign_kernel, in `d_img` for host storage (the rows a push wrote are then
 // copied back) or straight into the caller's device storage.

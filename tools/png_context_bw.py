@@ -11,7 +11,7 @@ into host storage.  Per mode: the whole decode's time, per-push latency (median 
 a push returns once the storage holds its rows) and kernel launches per push.  Every mode's final storage is checked
 against png_decode_batch's.  The card's name and power limit are printed first.
 
-    python tools/png_context_bw.py [--repeat 3] [--out FILE]
+    python tools/png_context_bw.py [--repeat 3] [--out FILE] [--modes chunks,...] [--cache DIR]
 """
 import argparse
 import concurrent.futures
@@ -63,6 +63,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--repeat", type=int, default=3)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--cache", default=None, help="directory that keeps the two files between runs")
+    ap.add_argument("--modes", default="chunks,chunks+overdraw,one push,one push+overdraw",
+                    help="comma-separated online modes to time (a slow build may time only some)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("no CUDA device: nothing to measure")
@@ -72,8 +75,15 @@ def main():
     ctx = pkg.Context(0)
     img = corpus.make("photo", W, H, 11).tobytes()
     fmt = oracle.make_format(6, 8)
-    with concurrent.futures.ThreadPoolExecutor(2) as pool:
-        files = list(pool.map(lambda il: oracle.png_compress(img, W, H, fmt, il, 9, 65544), (False, True)))
+    cached = [os.path.join(args.cache, f"8k_{n}.png") for n in ("plain", "adam7")] if args.cache else []
+    if cached and all(os.path.exists(p) for p in cached):
+        files = [open(p, "rb").read() for p in cached]
+    else:
+        with concurrent.futures.ThreadPoolExecutor(2) as pool:
+            files = list(pool.map(lambda il: oracle.png_compress(img, W, H, fmt, il, 9, 65544), (False, True)))
+        for p, f in zip(cached, files):
+            os.makedirs(args.cache, exist_ok=True)
+            open(p, "wb").write(f)
     rows = []
     for interlaced, f in zip((False, True), files):
         chunks = pngio.idat_chunks(f)
@@ -82,6 +92,7 @@ def main():
         assert ref.status == 0 and ref.storage == img
         modes = [("chunks", chunks, False), ("chunks+overdraw", chunks, True),
                  ("one push", [whole], False), ("one push+overdraw", [whole], True)]
+        modes = [m for m in modes if m[0] in args.modes.split(",")]
         for name, pieces, od in modes:   # warm-up: every shape the timed runs use
             online(pkg, ctx, pieces[:3], interlaced, od, finish=False)
         pkg.png_decode_batch(ctx, [f])
