@@ -431,12 +431,34 @@ void   pngb200_inflator_error(const pngb200_inflator* z, int* status, uint32_t* 
  * twice), out[1] output bytes written (likewise), out[2] of those written by the one-warp serial decoder. */
 int    pngb200_inflator_stats(const pngb200_inflator* z, uint64_t out[3]);
 
+/* Many pushes in one call: the throughput path of the streaming handles, for a caller that holds many streams at once.
+ * Each item behaves exactly as the same push made alone through pngb200_inflator_push: its status, error payload,
+ * available bytes, pulled bytes and stats are the ones that push would leave, whatever else the call holds.  The handles
+ * are distinct, so item order does not matter.  Terminal handles and handles with a sticky error are answered on the
+ * host, with no device work.  Items may mix formats.  Usable while a decode batch is pending on the ctx (the pushes
+ * have workspaces of their own).
+ * Returns PNGB200_OK once every item's status is written, even when some items failed; PNGB200_ERR_BAD_ARGUMENT, before
+ * any work and with no item touched, for a null ctx, pushes NULL with count > 0, a null handle, a handle of another ctx,
+ * the same handle twice, or data NULL with n > 0 (count == 0 is OK); PNGB200_ERR_CUDA on a CUDA failure, each item not
+ * finished then left as a single push failing the same way would leave it (status PNGB200_ERR_CUDA).
+ * Fixed cost, whatever `count`: one round of at most 2 kernel launches (the ring inflate kernel over the items with
+ * 64 KiB or more of undecoded input, the serial one over the rest) and 1 stream synchronise, then, when streams ended,
+ * 2 checksum launches and 1 synchronise.  An item whose output buffer has to grow goes again in a further round, with
+ * the other items of that kind only: each such round adds the same costs. */
+typedef struct pngb200_inflator_push_desc {
+    pngb200_inflator* inflator;
+    const uint8_t*    data;      /* host memory, copied, as pngb200_inflator_push */
+    size_t            n;
+    int32_t           status;    /* out: what pngb200_inflator_push would return for this push */
+} pngb200_inflator_push_desc;
+int    pngb200_inflator_push_batch(pngb200_ctx* ctx, pngb200_inflator_push_desc* pushes, size_t count);
+
 /* ---- online decoding: PNG.Context (Sources/PNG/Decoding/PNG.Context.swift) ----------------------------------------
  * A caller pushes each IDAT chunk as it arrives; after every push the storage is a valid partial image.  Restates
  * PNG.Context.push(data:overdraw:), the row state machine of PNG.Decoder.push (PNG.Decoder.swift:47-149),
  * PNG.Image.assign and PNG.Image.overdraw (PNG.Image.swift:133-285), and push(ancillary:) with IEND.
  * Inflate runs on the device through a pngb200_inflator; the newly available scanlines are reconstructed by
- * unfilter_pass_kernel and written into storage, pass by pass, by context_assign_kernel.  After each push the rows
+ * unfilter_pass_kernel and written into storage, pass by pass, by context_assign_batch_kernel.  After each push the rows
  * assigned are exactly the reference's: its inflator releases the payload of a stored block as it arrives, and so
  * does the context (the pngb200_inflator handle itself waits for the whole block). */
 typedef struct pngb200_png_context pngb200_png_context;
@@ -463,6 +485,27 @@ pngb200_png_context* pngb200_png_context_create(pngb200_ctx* ctx, const pngb200_
  * `overdraw` each scanline is overdrawn right after it is assigned (it may differ from one push to the next).  The call
  * returns once the storage holds the new rows, host or device. */
 int  pngb200_png_context_push(pngb200_png_context* c, const uint8_t* data, size_t n, int overdraw);
+
+/* Many pushes in one call, one per context: the throughput path for a caller with many images in flight.  Each item
+ * behaves exactly as the same push made alone through pngb200_png_context_push: its status, error payload, progress
+ * (all six values) and storage are the ones that push would leave.  The contexts are distinct, so item order does not
+ * matter; each keeps the stored-block rule (a stored block's payload is released as it arrives).  Terminal contexts
+ * and contexts with a sticky error are answered on the host, with no device work.  Items may mix storage memspaces,
+ * standards, interlacing, depths, volumes and overdraw.
+ * Returns and rejects as pngb200_inflator_push_batch, and also rejects (PNGB200_ERR_BAD_ARGUMENT, no item touched) a
+ * call while a decode batch is pending on the ctx.
+ * Fixed cost, whatever `count`: the inflator rounds of pngb200_inflator_push_batch, then 1 unfilter_pass_kernel launch
+ * over the new rows of every context, at most 7 context_assign_batch_kernel launches (launch k assigns the k-th pass
+ * range every context touched in this push) and 1 stream synchronise.  pngb200_png_context_push is this call with
+ * one item. */
+typedef struct pngb200_png_push_desc {
+    pngb200_png_context* context;
+    const uint8_t*       data;   /* host memory: one IDAT payload, any length, empty included */
+    size_t               n;
+    int32_t              overdraw;
+    int32_t              status; /* out: what pngb200_png_context_push would return for this push */
+} pngb200_png_push_desc;
+int  pngb200_png_context_push_batch(pngb200_ctx* ctx, pngb200_png_push_desc* pushes, size_t count);
 /* push(ancillary:) with IEND: PNGB200_OK if and only if the DEFLATE stream is complete, else
  * PNGB200_ERR_PNG_INCOMPLETE_DATASTREAM.  A complete stream with too few rows is OK, as in pngb200_decode_batch. */
 int  pngb200_png_context_end(pngb200_png_context* c);

@@ -44,15 +44,57 @@ extension PNG
             {
                 pngb200_png_context_push(self.handle, $0.baseAddress, $0.count, overdraw ? 1 : 0)
             }
+            if let error:any Error = self.error(status: status)
+            {
+                throw error
+            }
+        }
+
+        /// Many pushes in one call (pngb200_png_context_push_batch), one per context, each context at most once: for a
+        /// caller with many images in flight.  Returns, per push, the error push(data:overdraw:) would throw for it, or
+        /// nil; throws only when the call itself fails.
+        static
+        func push(_ pushes:[(context:DeviceContext, data:[UInt8], overdraw:Bool)]) throws -> [(any Error)?]
+        {
+            let bytes:[UInt8] = pushes.flatMap(\.data)
+            var descs:[pngb200_png_push_desc] = []
+            let status:Int32 = bytes.withUnsafeBufferPointer
+            {
+                (bytes:UnsafeBufferPointer<UInt8>) in
+                var offset:Int = 0
+                for push:(context:DeviceContext, data:[UInt8], overdraw:Bool) in pushes
+                {
+                    var desc:pngb200_png_push_desc = .init()
+                    desc.context  = push.context.handle
+                    desc.data     = bytes.baseAddress.map { $0 + offset }
+                    desc.n        = push.data.count
+                    desc.overdraw = push.overdraw ? 1 : 0
+                    descs.append(desc)
+                    offset       += push.data.count
+                }
+                return pngb200_png_context_push_batch(LZ77.GPU.shared.ctx, &descs, descs.count)
+            }
+            guard status == 0
+            else
+            {
+                throw pngb200Error(status: status, 0, 0)
+            }
+            return zip(pushes, descs).map { $0.context.error(status: $1.status) }
+        }
+
+        /// the error push(data:overdraw:) throws for a push status, or nil
+        private
+        func error(status:Int32) -> (any Error)?
+        {
             switch status
             {
-            case 0:     return
-            case -48:   throw PNG.DecodingError.extraneousImageData                      // PNG.Decoder.swift:142-147
-            case -49:   throw PNG.DecodingError.extraneousImageDataCompressedData         // :51-55
+            case 0:     return nil
+            case -48:   return PNG.DecodingError.extraneousImageData                      // PNG.Decoder.swift:142-147
+            case -49:   return PNG.DecodingError.extraneousImageDataCompressedData         // :51-55
             default:
                 var s:Int32 = 0, a:UInt32 = 0, b:UInt32 = 0
                 pngb200_png_context_error(self.handle, &s, &a, &b)
-                throw pngb200Error(status: status, a, b)                                  // LZ77 errors, as the inflator
+                return pngb200Error(status: status, a, b)                                 // LZ77 errors, as the inflator
             }
         }
 

@@ -178,6 +178,15 @@ class PngContextDesc(C.Structure):
     ]
 
 
+class InflatorPushDesc(C.Structure):
+    _fields_ = [("inflator", C.c_void_p), ("data", C.c_void_p), ("n", C.c_size_t), ("status", C.c_int32)]
+
+
+class PngPushDesc(C.Structure):
+    _fields_ = [("context", C.c_void_p), ("data", C.c_void_p), ("n", C.c_size_t), ("overdraw", C.c_int32),
+                ("status", C.c_int32)]
+
+
 class PNGB200Error(RuntimeError):
     def __init__(self, status: int, message: str = ""):
         super().__init__(f"pngb200 status {status}: {message}")
@@ -317,6 +326,11 @@ def lib():
         L.pngb200_png_context_error.restype = None
         L.pngb200_png_context_destroy.argtypes = [C.c_void_p]
         L.pngb200_png_context_destroy.restype = None
+    if os.environ.get("PNGB200_LIB") is None or hasattr(L, "pngb200_png_context_push_batch"):   # (older builds lack it)
+        L.pngb200_inflator_push_batch.argtypes = [C.c_void_p, C.POINTER(InflatorPushDesc), C.c_size_t]
+        L.pngb200_inflator_push_batch.restype = C.c_int
+        L.pngb200_png_context_push_batch.argtypes = [C.c_void_p, C.POINTER(PngPushDesc), C.c_size_t]
+        L.pngb200_png_context_push_batch.restype = C.c_int
     _lib = L
     return L
 
@@ -876,6 +890,12 @@ class Inflator:
             raise e
         return st
 
+    def error(self):
+        """(sticky status, payload a, payload b): PNGB200_NEED_MORE_INPUT or OK while there is no error"""
+        s, a, b = C.c_int(), C.c_uint32(), C.c_uint32()
+        self.ctx._lib.pngb200_inflator_error(self.handle, C.byref(s), C.byref(a), C.byref(b))
+        return s.value, a.value, b.value
+
     def pull(self, count: int):
         """Exactly `count` bytes or None (Swift: pull(_:) -> [UInt8]?)."""
         buf = C.create_string_buffer(max(count, 1))
@@ -937,6 +957,12 @@ class PngContext:
             e.payload = (a.value, b.value) if s.value == st else (0, 0)
             raise e
 
+    def error(self):
+        """(sticky inflate status, payload a, payload b): OK while there is no error"""
+        s, a, b = C.c_int(), C.c_uint32(), C.c_uint32()
+        self.ctx._lib.pngb200_png_context_error(self.handle, C.byref(s), C.byref(a), C.byref(b))
+        return s.value, a.value, b.value
+
     def end(self) -> None:
         """push(ancillary:) with IEND: raises PNGB200Error(ERR_PNG_INCOMPLETE_DATASTREAM) unless the stream is complete"""
         st = self.ctx._lib.pngb200_png_context_end(self.handle)
@@ -952,3 +978,34 @@ class PngContext:
     def storage(self):
         """host storage: its bytes; device storage: its address"""
         return C.string_at(self._addr, self._size) if self._host is not None else self._addr
+
+
+
+def _push_batch(ctx: Context, kind, entry, items):
+    """one batch push of `items` (handle, data[, overdraw]); returns the per-item statuses"""
+    descs = (kind * max(len(items), 1))()
+    keep = []   # the bytes the descriptors point into
+    for d, item in zip(descs, items):
+        data = bytes(item[1])
+        keep.append(data)
+        setattr(d, kind._fields_[0][0], item[0].handle)
+        d.data = C.cast(C.c_char_p(data), C.c_void_p)
+        d.n = len(data)
+        if kind is PngPushDesc:
+            d.overdraw = int(item[2])
+    ctx.check(entry(ctx.handle, descs, len(items)))
+    return [descs[i].status for i in range(len(items))]
+
+
+def inflator_push_batch(ctx: Context, items) -> list:
+    """push(_:) of many Inflators in one call: `items` is [(inflator, data)], distinct inflators of `ctx`.  Returns
+    each push's status, as Inflator.push would return or raise it (payloads through the inflator's error()); raises
+    PNGB200Error only when the call itself fails."""
+    return _push_batch(ctx, InflatorPushDesc, ctx._lib.pngb200_inflator_push_batch, items)
+
+
+def png_context_push_batch(ctx: Context, items) -> list:
+    """push(data:overdraw:) of many PngContexts in one call: `items` is [(png_context, data, overdraw)], distinct
+    contexts of `ctx`.  Returns each push's status, as PngContext.push would raise it (payloads through the context's
+    error()); raises PNGB200Error only when the call itself fails."""
+    return _push_batch(ctx, PngPushDesc, ctx._lib.pngb200_png_context_push_batch, items)

@@ -112,6 +112,10 @@ struct pngb200_ctx {
            d_file, d_crc, d_seg, d_crctab, d_sgjobs, d_sgres, d_sgsym, d_sgsearch, d_sgrec, d_sgwin;
     // pinned host tables
     PinBuf h_jobs, h_results, h_imgjobs, h_genjobs, h_misc, h_order, h_crc, h_seg, h_sgsearch, h_sgjobs, h_sgres, h_sgrec;
+    // the streaming handles' pushes (pngb200_inflator_push_batch, pngb200_png_context_push_batch): tables, checksum
+    // bases and partials, and the staged input, apart from the decode batch's so that they may run while one is pending
+    DevBuf d_st, d_stbase, d_stpartial, d_stin;
+    PinBuf h_st, h_stin;
     uint64_t seg_streams = 0, seg_segments = 0, seg_fallbacks = 0;  // last batch: streams cut into segments, segments, rejected
     uint64_t split_stats[6] = {};      // last batch, streams cut in two: see pngb200_ctx_split_stats
     uint64_t scratch_stride = 0;       // layout of d_scratch the last inflate launch used
@@ -1836,8 +1840,7 @@ struct pngb200_inflator {
     pngb200_ctx*         ctx;
     int                  format;
     std::vector<uint8_t> input;      // everything pushed so far
-    DevBuf               d_in, d_out, d_job, d_res, d_misc, d_partial;
-    PinBuf               h_res;
+    DevBuf               d_in, d_out;
     size_t               uploaded = 0;
     uint64_t             resume_bit = 0, resume_out = 0, produced = 0, current = 0;
     uint32_t             phase = 0;
@@ -1865,107 +1868,214 @@ void pngb200_inflator_destroy(pngb200_inflator* z)
     delete z;   // frees the workspaces
 }
 
-static int inflator_grow_out(pngb200_inflator* z, size_t need)
+}  // extern "C"
+
+namespace {
+
+// Grows a device buffer to at least `need` bytes, carrying its first `keep` bytes over device to device.  The old
+// memory goes to `retired`, which the caller frees once the stream has passed the copy.
+int grow_carrying(pngb200_ctx* ctx, DevBuf& b, size_t need, size_t keep, std::vector<DevBuf>& retired)
 {
-    pngb200_ctx* ctx = z->ctx;
-    if (need <= z->d_out.cap) return PNGB200_OK;
+    if (need <= b.cap) return PNGB200_OK;
     DevBuf bigger;
-    CU(bigger.reserve(std::max(need, z->d_out.cap * 2)));
-    cudaError_t e = cudaSuccess;
-    if (z->produced) e = cudaMemcpyAsync(bigger.p, z->d_out.p, z->produced, cudaMemcpyDeviceToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) return set_error(ctx, PNGB200_ERR_CUDA, "inflator: growing the output failed: %s", cudaGetErrorString(e));
-    z->d_out = std::move(bigger);   // the old output goes with `bigger`
+    CU(bigger.reserve(need));
+    if (keep) CU(cudaMemcpyAsync(bigger.p, b.p, keep, cudaMemcpyDeviceToDevice, ctx->stream));
+    std::swap(b, bigger);
+    retired.push_back(std::move(bigger));
     return PNGB200_OK;
+}
+
+// The pushes of one pngb200_inflator_push_batch call, on distinct handles of `ctx`.  Every item's `status` is
+// PNGB200_ERR_CUDA until its push is answered, so that a CUDA failure leaves the items it stopped as a single push that
+// failed the same way.  `retired`: buffers the caller frees after its final stream synchronise.
+int inflate_pushes(pngb200_ctx* ctx, pngb200_inflator_push_desc* const* items, size_t count, std::vector<DevBuf>& retired)
+{
+    std::vector<pngb200_inflator_push_desc*> live;
+    size_t staged = 0;
+    for (size_t i = 0; i < count; ++i) {
+        pngb200_inflator_push_desc* d = items[i];
+        pngb200_inflator* z = d->inflator;
+        if (z->terminal) d->status = PNGB200_OK;   // LZ77.Inflator ignores input after the terminal state
+        else if (z->status < 0) d->status = z->status;
+        else {
+            d->status = PNGB200_ERR_CUDA;
+            live.push_back(d);
+            staged += d->n;
+        }
+    }
+    if (live.empty()) return PNGB200_OK;
+    // the new input of every handle: one upload into staging, then appended to each handle's device copy
+    if (staged) {
+        CU(ctx->h_stin.reserve(staged));
+        CU(ctx->d_stin.reserve(staged));
+        size_t off = 0;
+        for (pngb200_inflator_push_desc* d : live)
+            if (d->n) memcpy(ctx->h_stin.as<uint8_t>() + off, d->data, d->n), off += d->n;
+        CU(cudaMemcpyAsync(ctx->d_stin.p, ctx->h_stin.p, staged, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    size_t off = 0;
+    for (pngb200_inflator_push_desc* d : live) {
+        pngb200_inflator* z = d->inflator;
+        z->input.insert(z->input.end(), d->data, d->data + d->n);
+        if (z->input.size() + 16 > z->d_in.cap)   // 16 bytes of slack behind the input for the decoders' bit reader
+            if (int rc = grow_carrying(ctx, z->d_in, z->input.size() * 2 + 4096, z->uploaded, retired)) return rc;
+        if (d->n)
+            CU(cudaMemcpyAsync(z->d_in.as<uint8_t>() + z->uploaded, ctx->d_stin.as<uint8_t>() + off, d->n,
+                               cudaMemcpyDeviceToDevice, ctx->stream));
+        off += d->n;
+        z->uploaded = z->input.size();
+        const size_t want = std::max<size_t>(1 << 16, z->produced + 4 * d->n + 1024);
+        if (want > z->d_out.cap)
+            if (int rc = grow_carrying(ctx, z->d_out, std::max(want, z->d_out.cap * 2), z->produced, retired)) return rc;
+    }
+    // Rounds: every live handle decodes once; a handle whose output ran out grows it and goes again in the next round.
+    constexpr uint64_t kWave = 64u << 10;
+    std::vector<pngb200_inflator_push_desc*> round = live;
+    while (!round.empty()) {
+        // A push with a lot of undecoded input goes through the intra-stream parallel kernel (one CTA: ~25 x the
+        // lock-step warp); short ones, and what is left of the wave the input ends in, through the serial decoder.
+        // Both resume where the last push stopped: at a block header, or at the last complete symbol of a Huffman block.
+        auto pending = [](const pngb200_inflator* z) {
+            return z->input.size() - std::min<uint64_t>(z->input.size(), z->resume_bit >> 3);
+        };
+        std::stable_partition(round.begin(), round.end(),
+                              [&](const pngb200_inflator_push_desc* d) { return pending(d->inflator) >= kWave; });
+        const size_t m = round.size();
+        size_t big = 0;
+        uint64_t max_cap = 0;
+        std::vector<StreamJob>    jobs(m);
+        std::vector<StreamResult> res(m);
+        std::vector<ResumePoint>  at(m);
+        for (size_t k = 0; k < m; ++k) {
+            pngb200_inflator* z = round[k]->inflator;
+            jobs[k] = whole_stream_job(z->d_in.as<uint8_t>(), z->input.size(), z->d_out.as<uint8_t>(), z->d_out.cap, z->format);
+            jobs[k].start_bit = z->resume_bit;
+            jobs[k].start_out = z->resume_out;
+            jobs[k].phase = (int32_t)z->phase;
+            memset(&res[k], 0, sizeof res[k]);
+            at[k] = z->at;
+            at[k].bits = at[k].bytes = at[k].serial_bytes = 0;
+            if (pending(z) >= kWave) big++, max_cap = std::max<uint64_t>(max_cap, z->d_out.cap);
+        }
+        Tables t(ctx->h_st, ctx->d_st);
+        const size_t off_jobs = t.host(jobs.data(), sizeof(StreamJob) * m);
+        const size_t off_res  = t.host(res.data(), sizeof(StreamResult) * m);
+        const size_t off_at   = t.host(at.data(), sizeof(ResumePoint) * m);
+        CU(ctx->d_st.reserve(t.end));   // now, so that the jobs can point at their resume records
+        for (size_t k = 0; k < m; ++k) jobs[k].resume = t.dev<ResumePoint>(off_at) + k;
+        if (int rc = t.upload(ctx)) return rc;
+        StreamJob*    d_jobs = t.dev<StreamJob>(off_jobs);
+        StreamResult* d_res  = t.dev<StreamResult>(off_res);
+        if (big) {
+            const unsigned grid = (unsigned)std::min<size_t>(big, 2 * (size_t)ctx->sm_count);
+            if (int rc = launch_waves(ctx, ENG_WAVE, d_jobs, d_res, nullptr, big, grid, max_cap, nullptr)) return rc;
+        }
+        if (m > big) {
+            inflate_serial_kernel<<<(unsigned)(m - big), 32, 0, ctx->stream>>>(d_jobs + big, d_res + big, nullptr, (int)(m - big));
+            ctx->launches++;
+        }
+        CU(cudaGetLastError());
+        // the results and the resume records lie side by side: one readback
+        CU(cudaMemcpyAsync(t.pin<char>(off_res), t.dev<char>(off_res), off_at + sizeof(ResumePoint) * m - off_res,
+                           cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        memcpy(res.data(), t.pin<StreamResult>(off_res), sizeof(StreamResult) * m);
+        memcpy(at.data(), t.pin<ResumePoint>(off_at), sizeof(ResumePoint) * m);
+        // The stream checksum is only due when the trailer has been read: ONE pass over the output at the end of the
+        // stream, not one per push, for every stream of the round that ended in it.
+        std::vector<size_t> ended;
+        for (size_t k = 0; k < m; ++k)
+            if (res[k].trailer_seen && !res[k].ck_done) ended.push_back(k);
+        if (!ended.empty()) {
+            const size_t e = ended.size();
+            std::vector<StreamJob>    ck_jobs(e);
+            std::vector<StreamResult> ck_res(e);
+            for (size_t i = 0; i < e; ++i) ck_jobs[i] = jobs[ended[i]], ck_res[i] = res[ended[i]];
+            Tables c(ctx->h_st, ctx->d_st);
+            const size_t off_cj = c.host(ck_jobs.data(), sizeof(StreamJob) * e);
+            const size_t off_cr = c.host(ck_res.data(), sizeof(StreamResult) * e);
+            if (int rc = c.upload(ctx)) return rc;
+            std::vector<uint32_t> base(e + 1);
+            if (int rc = run_checksum(ctx, ck_jobs.data(), c.dev<StreamJob>(off_cj), c.dev<StreamResult>(off_cr), e, base.data(),
+                                      ctx->d_stbase, ctx->d_stpartial))
+                return rc;
+            CU(cudaMemcpyAsync(c.pin<char>(off_cr), c.dev<char>(off_cr), sizeof(StreamResult) * e, cudaMemcpyDeviceToHost,
+                               ctx->stream));
+            CU(cudaStreamSynchronize(ctx->stream));
+            for (size_t i = 0; i < e; ++i) res[ended[i]] = c.pin<StreamResult>(off_cr)[i];
+        }
+        std::vector<pngb200_inflator_push_desc*> again;
+        for (size_t k = 0; k < m; ++k) {
+            pngb200_inflator* z = round[k]->inflator;
+            const StreamResult& r = res[k];
+            z->at = at[k];
+            z->work[0] += at[k].bits;
+            z->work[1] += at[k].bytes;
+            z->work[2] += at[k].serial_bytes;
+            // the next run resumes where this one stopped (after an output capacity error: where it started, or behind a
+            // block it completed)
+            z->phase = r.phase;
+            z->resume_bit = r.resume_bit;
+            z->resume_out = r.resume_out;
+            if (r.status == PNGB200_ERR_OUTPUT_CAPACITY) {
+                z->produced = r.resume_out;
+                if (int rc = grow_carrying(ctx, z->d_out, z->d_out.cap * 2, z->produced, retired)) return rc;
+                again.push_back(round[k]);
+                continue;
+            }
+            z->produced = r.produced;
+            z->status = r.status;
+            z->err_a = r.err_a;
+            z->err_b = r.err_b;
+            if (r.status == PNGB200_OK) z->terminal = true;
+            round[k]->status = r.status;
+        }
+        round.swap(again);
+    }
+    return PNGB200_OK;
+}
+
+// The call-level checks of both batch pushes: distinct handles of `ctx`, and data for every byte announced
+template <typename Desc, typename Handle>
+int check_pushes(pngb200_ctx* ctx, const Desc* pushes, size_t count, Handle* Desc::*handle, const char* what)
+{
+    if (!ctx || (!pushes && count)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "%s: null argument", what);
+    std::vector<const void*> seen(count);
+    for (size_t i = 0; i < count; ++i) {
+        const Handle* h = pushes[i].*handle;
+        if (!h || h->ctx != ctx || (!pushes[i].data && pushes[i].n))
+            return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "%s: item %zu has no handle of this context or no data", what, i);
+        seen[i] = h;
+    }
+    std::sort(seen.begin(), seen.end());
+    if (std::adjacent_find(seen.begin(), seen.end()) != seen.end())
+        return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "%s: a handle appears twice", what);
+    return PNGB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pngb200_inflator_push_batch(pngb200_ctx* ctx, pngb200_inflator_push_desc* pushes, size_t count)
+{
+    if (int rc = check_pushes(ctx, pushes, count, &pngb200_inflator_push_desc::inflator, "inflator_push_batch")) return rc;
+    if (!count) return PNGB200_OK;
+    DeviceGuard guard(ctx->device);
+    std::vector<pngb200_inflator_push_desc*> items(count);
+    for (size_t i = 0; i < count; ++i) items[i] = &pushes[i];
+    std::vector<DevBuf> retired;
+    const int rc = inflate_pushes(ctx, items.data(), count, retired);
+    if (rc != PNGB200_OK) cudaStreamSynchronize(ctx->stream);   // before `retired` frees what the stream may still read
+    return rc;
 }
 
 int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
 {
     if (!z || (!data && n)) return PNGB200_ERR_BAD_ARGUMENT;
-    pngb200_ctx* ctx = z->ctx;
-    if (z->terminal) return PNGB200_OK;  // LZ77.Inflator ignores input after the terminal state
-    if (z->status < 0) return z->status;
-    DeviceGuard guard(ctx->device);
-    z->input.insert(z->input.end(), data, data + n);
-    // device copy of the whole input (grow-only; new bytes appended)
-    if (z->input.size() + 16 > z->d_in.cap) {
-        DevBuf bigger;
-        CU(bigger.reserve(z->input.size() * 2 + 4096));
-        z->d_in = std::move(bigger);   // the old copy goes with `bigger`
-        z->uploaded = 0;
-    }
-    if (z->input.size() > z->uploaded)
-        CU(cudaMemcpyAsync(z->d_in.as<uint8_t>() + z->uploaded, z->input.data() + z->uploaded,
-                           z->input.size() - z->uploaded, cudaMemcpyHostToDevice, ctx->stream));
-    z->uploaded = z->input.size();
-    // d_res and h_res hold the result, then the resume record; h_res then stages the job
-    constexpr size_t kIo = sizeof(StreamResult) + sizeof(ResumePoint);
-    CU(z->d_job.reserve(sizeof(StreamJob)));
-    CU(z->d_res.reserve(kIo));
-    CU(z->h_res.reserve(kIo + sizeof(StreamJob)));
-    int rc = inflator_grow_out(z, std::max<size_t>(1 << 16, z->produced + 4 * n + 1024));
-    if (rc != PNGB200_OK) return rc;
-    for (;;) {
-        StreamResult* res = z->h_res.as<StreamResult>();
-        ResumePoint*  at  = reinterpret_cast<ResumePoint*>(res + 1);
-        StreamJob*    job = reinterpret_cast<StreamJob*>(at + 1);
-        *job = whole_stream_job(z->d_in.as<uint8_t>(), z->input.size(), z->d_out.as<uint8_t>(), z->d_out.cap, z->format);
-        job->start_bit = z->resume_bit;
-        job->start_out = z->resume_out;
-        job->phase = (int32_t)z->phase;
-        job->resume = reinterpret_cast<ResumePoint*>(z->d_res.as<StreamResult>() + 1);
-        memset(res, 0, sizeof *res);
-        *at = z->at;
-        at->bits = at->bytes = at->serial_bytes = 0;
-        CU(cudaMemcpyAsync(z->d_job.p, job, sizeof(StreamJob), cudaMemcpyHostToDevice, ctx->stream));
-        CU(cudaMemcpyAsync(z->d_res.p, res, kIo, cudaMemcpyHostToDevice, ctx->stream));
-        // A push with a lot of undecoded input goes through the intra-stream parallel kernel (one CTA: ~25 x the
-        // lock-step warp); short ones, and what is left of the wave the input ends in, through the serial decoder.
-        // Both resume where the last push stopped: at a block header, or at the last complete symbol of a Huffman block.
-        const uint64_t pending = z->input.size() - std::min<uint64_t>(z->input.size(), z->resume_bit >> 3);
-        if (pending >= (64u << 10)) {
-            rc = launch_waves(ctx, ENG_WAVE, z->d_job.as<StreamJob>(), z->d_res.as<StreamResult>(), nullptr, 1, 1, job->dst_cap, nullptr);
-            if (rc != PNGB200_OK) return rc;
-        } else {
-            inflate_serial_kernel<<<1, 32, 0, ctx->stream>>>(z->d_job.as<StreamJob>(), z->d_res.as<StreamResult>(), nullptr, 1);
-            ctx->launches++;
-        }
-        CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(z->h_res.p, z->d_res.p, kIo, cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        // The stream checksum is only due when the trailer has been read: ONE pass over the output at the end of the
-        // stream, not one per push (round 1 re-checksummed everything produced so far on every push).
-        if (z->h_res.as<StreamResult>()->trailer_seen && !z->h_res.as<StreamResult>()->ck_done) {
-            // the inflator's own tables: it may run while a decode batch is pending on the context
-            uint32_t base[2];
-            rc = run_checksum(ctx, job, z->d_job.as<StreamJob>(), z->d_res.as<StreamResult>(), 1, base, z->d_misc, z->d_partial);
-            if (rc != PNGB200_OK) return rc;
-            CU(cudaMemcpyAsync(z->h_res.p, z->d_res.p, sizeof(StreamResult), cudaMemcpyDeviceToHost, ctx->stream));
-            CU(cudaStreamSynchronize(ctx->stream));
-        }
-        const StreamResult r = *res;
-        z->at = *at;
-        z->work[0] += at->bits;
-        z->work[1] += at->bytes;
-        z->work[2] += at->serial_bytes;
-        // the next run resumes where this one stopped (after an output capacity error: where it started, or behind a
-        // block it completed)
-        z->phase = r.phase;
-        z->resume_bit = r.resume_bit;
-        z->resume_out = r.resume_out;
-        if (r.status == PNGB200_ERR_OUTPUT_CAPACITY) {
-            z->produced = r.resume_out;
-            rc = inflator_grow_out(z, z->d_out.cap * 2);
-            if (rc != PNGB200_OK) return rc;
-            continue;
-        }
-        z->produced = r.produced;
-        z->status = r.status;
-        z->err_a = r.err_a;
-        z->err_b = r.err_b;
-        if (r.status == PNGB200_OK) z->terminal = true;
-        return r.status;
-    }
+    pngb200_inflator_push_desc d{z, data, n, 0};
+    const int rc = pngb200_inflator_push_batch(z->ctx, &d, 1);
+    return rc != PNGB200_OK ? rc : d.status;
 }
 
 size_t pngb200_inflator_available(const pngb200_inflator* z) { return z ? (size_t)(z->produced - z->current) : 0; }
@@ -2022,8 +2132,7 @@ struct pngb200_png_context {
     uint8_t*          pixels = nullptr;   // the caller's storage
     uint64_t          storage = 0;        // its bytes
     uint64_t          fsize = 0;          // filtered bytes of the image
-    DevBuf            d_img, d_filt, d_jobs;
-    PinBuf            h_jobs;
+    DevBuf            d_img, d_filt;
     uint64_t          copied = 0;         // bytes of d_filt filled
     uint64_t          drained = 0;        // bytes the decoder has pulled once every row was assigned
     int               pass = 0;           // next pass, 7 once every row is assigned (PNG.Decoder.pass)
@@ -2109,79 +2218,142 @@ static uint64_t stored_in_flight(const pngb200_inflator* z, uint64_t* src)
     return std::min<uint64_t>(len, in.size() - *src);
 }
 
-int pngb200_png_context_push(pngb200_png_context* c, const uint8_t* data, size_t n, int overdraw)
+}  // extern "C"
+
+namespace {
+
+// One push of pngb200_png_context_push_batch: the pass rows it reconstructs and assigns, in pass order
+struct ContextRange { int z; uint64_t r0, r1; };
+
+// The pushes of one pngb200_png_context_push_batch call, on distinct contexts of `ctx`: every context inflates in one
+// inflate_pushes call, copies its newly available filtered bytes and runs the row state machine; then the rows of
+// every context are reconstructed by one unfilter_pass_kernel launch and assigned by at most seven
+// context_assign_batch_kernel launches, the k-th over the k-th pass range of every context.  Statuses as in
+// inflate_pushes.
+int context_pushes(pngb200_ctx* ctx, pngb200_png_push_desc* pushes, size_t count, std::vector<DevBuf>& retired)
 {
-    if (!c || (!data && n)) return PNGB200_ERR_BAD_ARGUMENT;
-    pngb200_ctx* ctx = c->ctx;
-    if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_context_push: a decode batch is pending");
-    c->band[0] = c->band[1] = 0;
-    if (c->status < 0) return c->status;
-    if (c->terminal) return PNGB200_ERR_PNG_EXTRANEOUS_COMPRESSED_DATA;   // PNG.Decoder.swift:51-55
-    DeviceGuard guard(ctx->device);
-    const int rc = pngb200_inflator_push(c->z, data, n);
-    if (rc < 0) {   // no row of this push is assigned
-        int s;
-        pngb200_inflator_error(c->z, &s, &c->err_a, &c->err_b);
-        if (s != rc) c->err_a = c->err_b = 0;   // not a stream error (CUDA, capacity): no payload
-        return c->status = rc;
-    }
-    c->terminal = rc == PNGB200_OK;
-    uint64_t src = 0;
-    const uint64_t decoded = c->z->produced;
-    const uint64_t avail = decoded + stored_in_flight(c->z, &src);
-    const uint64_t fill = std::min(avail, c->fsize);
-    uint8_t* filt = c->d_filt.as<uint8_t>();
-    if (fill > c->copied) {
-        const uint64_t a = std::min(fill, decoded);
-        if (a > c->copied)
-            CU(cudaMemcpyAsync(filt + c->copied, c->z->d_out.as<uint8_t>() + c->copied, a - c->copied,
-                               cudaMemcpyDeviceToDevice, ctx->stream));
-        const uint64_t b = std::max(c->copied, decoded);
-        if (fill > b)
-            CU(cudaMemcpyAsync(filt + b, c->z->d_in.as<uint8_t>() + src + (b - decoded), fill - b, cudaMemcpyDeviceToDevice,
-                               ctx->stream));
-        c->copied = fill;
-    }
-    // PNG.Decoder.push's row loop (PNG.Decoder.swift:58-140): every complete scanline, in pass order, from where the last
-    // push stopped.  The first row a pass resumes at is reconstructed again from the row above it, whose filter byte
-    // becomes None: that row already holds its pixels, so it comes out unchanged and serves as the row above.
-    struct Range { int z; uint64_t r0, r1; };
-    std::vector<Range>   ranges;
-    std::vector<PassJob> jobs;
-    const uint32_t bpp = (c->volume + 7) >> 3;
-    int z = c->pass;
-    for (; z < 7; ++z) {
-        const Pass ps = stream_pass(z, c->w, c->h, c->volume, c->interlaced);
-        if (ps.height == 0) continue;
-        const uint64_t off  = stream_pass_offset(z, c->w, c->h, c->volume, c->interlaced);
-        const uint64_t r0   = z == c->pass ? c->row : 0;
-        const uint64_t have = c->copied > off ? (c->copied - off) / (ps.pitch + 1) : 0;
-        const uint64_t r1   = std::min<uint64_t>(have, ps.height);
-        if (r1 > r0) {
-            const uint64_t start = r0 ? r0 - 1 : 0;
-            uint8_t* first = filt + off + start * (ps.pitch + 1);
-            if (r0) CU(cudaMemsetAsync(first, 0, 1, ctx->stream));
-            jobs.push_back({first, nullptr, (r1 - start) * (ps.pitch + 1), 0, (uint32_t)(r1 - start), (uint32_t)ps.pitch, bpp});
-            ranges.push_back({z, r0, r1});
-        }
-        if (r1 < ps.height) {
-            c->pass = z;
-            c->row = r1;
-            break;
+    std::vector<pngb200_png_push_desc*>      live;
+    std::vector<pngb200_inflator_push_desc>  zp;
+    for (size_t i = 0; i < count; ++i) {
+        pngb200_png_push_desc* d = &pushes[i];
+        pngb200_png_context*   c = d->context;
+        c->band[0] = c->band[1] = 0;
+        if (c->status < 0) d->status = c->status;
+        else if (c->terminal) d->status = PNGB200_ERR_PNG_EXTRANEOUS_COMPRESSED_DATA;   // PNG.Decoder.swift:51-55
+        else {
+            d->status = PNGB200_ERR_CUDA;
+            live.push_back(d);
+            zp.push_back({c->z, d->data, d->n, 0});
         }
     }
-    if (z == 7) {
-        c->pass = 7;
-        c->row = 0;
+    if (live.empty()) return PNGB200_OK;
+    std::vector<pngb200_inflator_push_desc*> zi(zp.size());
+    for (size_t k = 0; k < zp.size(); ++k) zi[k] = &zp[k];
+    const int irc = inflate_pushes(ctx, zi.data(), zi.size(), retired);
+    std::vector<pngb200_png_push_desc*>   rowed;    // the pushes whose inflate succeeded
+    std::vector<uint64_t>                 avail;    // filtered bytes the reference has released after each of them
+    std::vector<std::vector<ContextRange>> ranges;
+    std::vector<PassJob>                  jobs;
+    for (size_t k = 0; k < live.size(); ++k) {
+        pngb200_png_context* c  = live[k]->context;
+        const int            rc = zp[k].status;
+        if (rc < 0) {   // no row of this push is assigned
+            int s;
+            pngb200_inflator_error(c->z, &s, &c->err_a, &c->err_b);
+            if (s != rc) c->err_a = c->err_b = 0;   // not a stream error (CUDA, capacity): no payload
+            live[k]->status = c->status = rc;
+        } else if (irc == PNGB200_OK) {
+            c->terminal = rc == PNGB200_OK;
+            rowed.push_back(live[k]);
+        }
     }
-    uint8_t* img = c->memspace == PNGB200_MEM_HOST ? c->d_img.as<uint8_t>() : c->pixels;
+    if (irc != PNGB200_OK) return irc;
+    for (pngb200_png_push_desc* d : rowed) {
+        pngb200_png_context* c = d->context;
+        uint64_t src = 0;
+        const uint64_t decoded = c->z->produced;
+        avail.push_back(decoded + stored_in_flight(c->z, &src));
+        const uint64_t fill = std::min(avail.back(), c->fsize);
+        uint8_t* filt = c->d_filt.as<uint8_t>();
+        if (fill > c->copied) {
+            const uint64_t a = std::min(fill, decoded);
+            if (a > c->copied)
+                CU(cudaMemcpyAsync(filt + c->copied, c->z->d_out.as<uint8_t>() + c->copied, a - c->copied,
+                                   cudaMemcpyDeviceToDevice, ctx->stream));
+            const uint64_t b = std::max(c->copied, decoded);
+            if (fill > b)
+                CU(cudaMemcpyAsync(filt + b, c->z->d_in.as<uint8_t>() + src + (b - decoded), fill - b, cudaMemcpyDeviceToDevice,
+                                   ctx->stream));
+            c->copied = fill;
+        }
+        // PNG.Decoder.push's row loop (PNG.Decoder.swift:58-140): every complete scanline, in pass order, from where the
+        // last push stopped.  The first row a pass resumes at is reconstructed again from the row above it, whose filter
+        // byte becomes None: that row already holds its pixels, so it comes out unchanged and serves as the row above.
+        ranges.emplace_back();
+        const uint32_t bpp = (c->volume + 7) >> 3;
+        int z = c->pass;
+        for (; z < 7; ++z) {
+            const Pass ps = stream_pass(z, c->w, c->h, c->volume, c->interlaced);
+            if (ps.height == 0) continue;
+            const uint64_t off  = stream_pass_offset(z, c->w, c->h, c->volume, c->interlaced);
+            const uint64_t r0   = z == c->pass ? c->row : 0;
+            const uint64_t have = c->copied > off ? (c->copied - off) / (ps.pitch + 1) : 0;
+            const uint64_t r1   = std::min<uint64_t>(have, ps.height);
+            if (r1 > r0) {
+                const uint64_t start = r0 ? r0 - 1 : 0;
+                uint8_t* first = filt + off + start * (ps.pitch + 1);
+                if (r0) CU(cudaMemsetAsync(first, 0, 1, ctx->stream));
+                jobs.push_back({first, nullptr, (r1 - start) * (ps.pitch + 1), 0, (uint32_t)(r1 - start), (uint32_t)ps.pitch, bpp});
+                ranges.back().push_back({z, r0, r1});
+            }
+            if (r1 < ps.height) {
+                c->pass = z;
+                c->row = r1;
+                break;
+            }
+        }
+        if (z == 7) {
+            c->pass = 7;
+            c->row = 0;
+        }
+        if (!ranges.back().empty()) c->band[0] = c->h;
+    }
+    // Assign launch k takes the k-th pass range of every context: the passes of one context stay in order (a later pass
+    // paints over an earlier one), and different contexts share no storage.
+    std::vector<AssignJob> assign[7];
+    std::vector<uint32_t>  cta_base[7];
+    uint32_t               ctas[7] = {};
+    for (size_t k = 0; k < 7; ++k) {
+        std::vector<AssignRange> rk;
+        std::vector<pngb200_png_context*> owner;
+        for (size_t i = 0; i < rowed.size(); ++i) {
+            if (ranges[i].size() <= k) continue;
+            pngb200_png_context* c = rowed[i]->context;
+            const ContextRange&  r = ranges[i][k];
+            rk.push_back({r.z, r.r0, r.r1, c->d_filt.as<uint8_t>(), c->memspace == PNGB200_MEM_HOST ? c->d_img.as<uint8_t>() : c->pixels,
+                          c->w, c->h, c->volume, c->depth, c->interlaced, rowed[i]->overdraw != 0});
+            owner.push_back(c);
+        }
+        if (rk.empty()) break;
+        std::vector<uint64_t> y;
+        ctas[k] = plan_assign_batch(rk, (unsigned)ctx->sm_count * 16, assign[k], cta_base[k], y);
+        for (size_t i = 0; i < owner.size(); ++i) {
+            owner[i]->band[0] = std::min(owner[i]->band[0], y[2 * i]);
+            owner[i]->band[1] = std::max(owner[i]->band[1], y[2 * i + 1]);
+        }
+    }
     if (!jobs.empty()) {
         std::vector<uint32_t> band_base, level_start;
         const uint64_t bands = plan_bands(jobs, band_base, level_start);
-        Tables t(c->h_jobs, c->d_jobs);
+        Tables t(ctx->h_st, ctx->d_st);
         const size_t off_jobs = t.host(jobs.data(), sizeof(PassJob) * jobs.size());
         const size_t off_bb = t.host(band_base.data(), sizeof(uint32_t) * band_base.size());
         const size_t off_ls = t.host(level_start.data(), sizeof(uint32_t) * level_start.size());
+        size_t off_aj[7], off_cb[7];
+        for (size_t k = 0; k < 7 && ctas[k]; ++k) {
+            off_aj[k] = t.host(assign[k].data(), sizeof(AssignJob) * assign[k].size());
+            off_cb[k] = t.host(cta_base[k].data(), sizeof(uint32_t) * cta_base[k].size());
+        }
         const size_t off_pr = t.device(sizeof(uint32_t) * (bands + 1), true);   // per-band progress, then the ticket
         if (int e = t.upload(ctx)) return e;
         WaveParams p;
@@ -2198,33 +2370,56 @@ int pngb200_png_context_push(pngb200_png_context* c, const uint8_t* data, size_t
         unfilter_pass_kernel<<<grid, WAVE_WARPS * 32, WAVE_SMEM, ctx->stream>>>(p);
         ctx->launches++;
         CU(cudaGetLastError());
-        // one launch per pass, in pass order: a later pass paints over an earlier one
-        c->band[0] = c->h;
-        for (const Range& r : ranges) {
-            AssignJob j;
-            uint64_t  y0, y1;
-            const uint32_t ctas = plan_assign(r.z, r.r0, r.r1, filt, img, c->w, c->h, c->volume, c->depth, c->interlaced,
-                                              overdraw != 0, (unsigned)ctx->sm_count * 16, &j, &y0, &y1);
-            context_assign_kernel<<<ctas, ASSIGN_THREADS, 0, ctx->stream>>>(j);
+        for (size_t k = 0; k < 7 && ctas[k]; ++k) {
+            context_assign_batch_kernel<<<ctas[k], ASSIGN_THREADS, 0, ctx->stream>>>(t.dev<AssignJob>(off_aj[k]), t.dev<uint32_t>(off_cb[k]),
+                                                                                   (uint32_t)assign[k].size());
             ctx->launches++;
             CU(cudaGetLastError());
-            c->band[0] = std::min(c->band[0], y0);
-            c->band[1] = std::max(c->band[1], y1);
         }
-        if (c->memspace == PNGB200_MEM_HOST) {
-            const uint64_t pitch = (uint64_t)c->w * bpp;
-            CU(cudaMemcpyAsync(c->pixels + c->band[0] * pitch, img + c->band[0] * pitch, (c->band[1] - c->band[0]) * pitch,
-                               cudaMemcpyDeviceToHost, ctx->stream));
-        }
+    }
+    for (pngb200_png_push_desc* d : rowed) {   // host storage: the rows the push wrote
+        pngb200_png_context* c = d->context;
+        if (c->memspace != PNGB200_MEM_HOST || c->band[1] <= c->band[0]) continue;
+        const uint64_t pitch = (uint64_t)c->w * ((c->volume + 7) >> 3);
+        CU(cudaMemcpyAsync(c->pixels + c->band[0] * pitch, c->d_img.as<uint8_t>() + c->band[0] * pitch,
+                           (c->band[1] - c->band[0]) * pitch, cudaMemcpyDeviceToHost, ctx->stream));
     }
     CU(cudaStreamSynchronize(ctx->stream));
-    // every row is assigned: any filtered byte beyond them is an error, in this push and in any later one
-    // (PNG.Decoder.swift:142-147; the bytes are drained, as inflator.pull() drains them)
-    if (c->pass == 7 && avail > c->drained) {
-        c->drained = avail;
-        return PNGB200_ERR_PNG_EXTRANEOUS_IMAGE_DATA;
+    for (size_t i = 0; i < rowed.size(); ++i) {
+        pngb200_png_context* c = rowed[i]->context;
+        rowed[i]->status = PNGB200_OK;
+        // every row is assigned: any filtered byte beyond them is an error, in this push and in any later one
+        // (PNG.Decoder.swift:142-147; the bytes are drained, as inflator.pull() drains them)
+        if (c->pass == 7 && avail[i] > c->drained) {
+            c->drained = avail[i];
+            rowed[i]->status = PNGB200_ERR_PNG_EXTRANEOUS_IMAGE_DATA;
+        }
     }
     return PNGB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pngb200_png_context_push_batch(pngb200_ctx* ctx, pngb200_png_push_desc* pushes, size_t count)
+{
+    if (int rc = check_pushes(ctx, pushes, count, &pngb200_png_push_desc::context, "png_context_push_batch")) return rc;
+    if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_context_push: a decode batch is pending");
+    if (!count) return PNGB200_OK;
+    DeviceGuard guard(ctx->device);
+    std::vector<DevBuf> retired;
+    const int rc = context_pushes(ctx, pushes, count, retired);
+    if (rc != PNGB200_OK) cudaStreamSynchronize(ctx->stream);   // before `retired` frees what the stream may still read
+    return rc;
+}
+
+int pngb200_png_context_push(pngb200_png_context* c, const uint8_t* data, size_t n, int overdraw)
+{
+    if (!c || (!data && n)) return PNGB200_ERR_BAD_ARGUMENT;
+    pngb200_png_push_desc d{c, data, n, overdraw, 0};
+    const int rc = pngb200_png_context_push_batch(c->ctx, &d, 1);
+    return rc != PNGB200_OK ? rc : d.status;
 }
 
 int pngb200_png_context_end(pngb200_png_context* c)

@@ -729,12 +729,14 @@ __host__ __device__ __forceinline__ void overdraw_brush(uint32_t bx, uint32_t ex
 // storage: the rectangles of one pass's rows are disjoint and a source is only ever written with its own value, which
 // is skipped, so no thread writes what another one reads.  Passes must still be launched in order: a later pass paints
 // over an earlier one.
-__global__ void __launch_bounds__(ASSIGN_THREADS) context_assign_kernel(AssignJob j)
+//
+// The job's tiles are shared by `ctas` CTAs, of which this is number `cta`.
+__device__ __forceinline__ void assign_tiles(const AssignJob& j, uint32_t cta, uint32_t ctas)
 {
     const uint32_t lper  = j.depth == 1 ? 3 : j.depth == 2 ? 2 : 1;
     const uint32_t sx    = 1u << j.ex;
     const uint32_t tiles = (j.r1 - j.r0) * j.tiles;   // plan_assign keeps the product below 2^32
-    for (uint32_t t = blockIdx.x; t < tiles; t += gridDim.x) {
+    for (uint32_t t = cta; t < tiles; t += ctas) {
         const uint32_t r    = j.r0 + t / j.tiles;
         const uint32_t tile = t % j.tiles;
         const uint64_t Y    = j.by + ((uint64_t)r << j.ey);
@@ -763,6 +765,22 @@ __global__ void __launch_bounds__(ASSIGN_THREADS) context_assign_kernel(AssignJo
             }
         }
     }
+}
+
+__global__ void __launch_bounds__(ASSIGN_THREADS) context_assign_kernel(AssignJob j) { assign_tiles(j, blockIdx.x, gridDim.x); }
+
+// Several AssignJobs in one launch, each of another image (two passes of one image must be launched one after the
+// other): job k runs on CTAs [cta_base[k], cta_base[k + 1]).
+__global__ void __launch_bounds__(ASSIGN_THREADS) context_assign_batch_kernel(const AssignJob* jobs, const uint32_t* cta_base,
+                                                                              uint32_t njobs)
+{
+    uint32_t lo = 0, hi = njobs;   // the last job whose first CTA is at or before this one
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) / 2;
+        if (cta_base[mid] <= blockIdx.x) lo = mid;
+        else hi = mid;
+    }
+    assign_tiles(jobs[lo], blockIdx.x - cta_base[lo], cta_base[lo + 1] - cta_base[lo]);
 }
 
 // The launch for rows [r0, r1) of pass z of an image whose filtered stream is at `filtered`, and the storage rows it
@@ -797,6 +815,34 @@ inline uint32_t plan_assign(int z, uint64_t r0, uint64_t r1, const uint8_t* filt
     *y0 = ps.by + (r0 << ps.ey);
     *y1 = overdraw && bw * bh > 1 ? std::min<uint64_t>(last + bh, h) : last + 1;
     return (uint32_t)std::min<uint64_t>(rows * j.tiles, max_ctas);
+}
+
+// Rows [r0, r1) of pass z of one image, for plan_assign_batch
+struct AssignRange {
+    int            z;
+    uint64_t       r0, r1;
+    const uint8_t* filtered;
+    uint8_t*       pixels;
+    uint32_t       w, h, volume, depth;
+    bool           interlaced, overdraw;
+};
+
+// One context_assign_batch_kernel launch over `ranges`, each of another image: every job is planned by plan_assign with
+// an equal share of the `max_ctas` budget (at least one CTA).  Fills jobs, cta_base (ranges.size() + 1 entries) and the
+// storage rows each range writes, y[2k] and y[2k + 1].  Returns the number of CTAs.
+inline uint32_t plan_assign_batch(const std::vector<AssignRange>& ranges, unsigned max_ctas, std::vector<AssignJob>& jobs,
+                                  std::vector<uint32_t>& cta_base, std::vector<uint64_t>& y)
+{
+    const unsigned share = std::max<unsigned>(1, max_ctas / (unsigned)std::max<size_t>(1, ranges.size()));
+    jobs.resize(ranges.size());
+    cta_base.assign(ranges.size() + 1, 0);
+    y.resize(2 * ranges.size());
+    for (size_t k = 0; k < ranges.size(); ++k) {
+        const AssignRange& a = ranges[k];
+        cta_base[k + 1] = cta_base[k] + plan_assign(a.z, a.r0, a.r1, a.filtered, a.pixels, a.w, a.h, a.volume, a.depth,
+                                                    a.interlaced, a.overdraw, share, &jobs[k], &y[2 * k], &y[2 * k + 1]);
+    }
+    return cta_base[ranges.size()];
 }
 
 }  // namespace pngb200
