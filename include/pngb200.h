@@ -522,14 +522,47 @@ void pngb200_png_context_destroy(pngb200_png_context* c);
  * init(format:level:exponent:hint:) -- `chunk_bytes` is the size of a complete output block: the reference hands out
  * 2 * capacity bytes, capacity being whatever malloc grants for `hint` UInt16 atoms (LZ77.DeflatorOut.swift:15-27,
  * 109-135); 0 = 65544, the value behind the reference's committed outputs (hint 1 << 15).
- * The device compresses a stream in one launch, so compressed blocks become available when push(last:) arrives;
- * pop() before that returns "nil" where the reference might already have a block.  The sequence of blocks a
- * caller sees -- sizes and bytes -- is the reference's. */
+ * Two constructors, which differ in *when* blocks become available, not in the bytes:
+ *  - pngb200_deflator_create: a buffered handle.  It keeps the input on the host and compresses the whole stream in
+ *    one launch at push(last: true), so pop() returns "nil" before that where the reference might already have a
+ *    block.
+ *  - pngb200_deflator_create_online: an online handle.  Each push does what LZ77.DeflatorBuffers.push(_:last:) does
+ *    (DeflatorBuffers.swift:68-137): when more than 4096 bytes are pending, or on `last`, deflate_resume_kernel
+ *    compresses on the device while more input than the lookahead (258; 259 for levels 4-7) is pending and writes
+ *    every block that fills; the state stays on the device between pushes.  After each push pop() / pull() return
+ *    exactly what the reference's would, with one deliberate difference: pull() before `last` returns a complete
+ *    block if there is one and otherwise nil, where the reference flushes a byte-padded partial block
+ *    (DeflatorOut.swift:96-101) that corrupts the rest of its stream.  The handle holds its dictionary (512 KiB), the
+ *    input from min(current block start, window start) on, and in full mode (levels 8-13) the unfinished block's
+ *    graph (128 bytes a vertex, at most 2^21 vertices), whatever the stream length.  One push is at most 1 GiB.
+ * With either, the sequence of blocks a caller sees -- sizes and bytes -- is the reference's. */
 typedef struct pngb200_deflator pngb200_deflator;
 pngb200_deflator* pngb200_deflator_create(pngb200_ctx* ctx, int format, int level, int exponent, size_t chunk_bytes);
+/* the same arguments and validation; NULL with PNGB200_ERR_CUDA in the last error if the device state cannot be had */
+pngb200_deflator* pngb200_deflator_create_online(pngb200_ctx* ctx, int format, int level, int exponent, size_t chunk_bytes);
 void              pngb200_deflator_destroy(pngb200_deflator* z);
-/* push(_:last:) : copies `data`.  Returns PNGB200_OK, or < 0 when compressing (on last) failed */
+/* push(_:last:) : copies `data`.  Returns PNGB200_OK, or < 0 when compressing failed.  A push after `last` is
+ * PNGB200_ERR_BAD_ARGUMENT.  On an online handle this is pngb200_deflator_push_batch with one item. */
 int    pngb200_deflator_push(pngb200_deflator* z, const uint8_t* data, size_t n, int last);
+/* push(_:last:) of many online handles in one call.  Each item behaves exactly as the same push made alone; items may
+ * mix formats, levels and exponents.  Returns PNGB200_ERR_BAD_ARGUMENT, touching no item, for a null ctx or array, a
+ * null handle, a buffered handle, a handle of another ctx, the same handle twice, data NULL with n > 0, or a pending
+ * decode batch; PNGB200_ERR_CUDA, with every handle unchanged, when a buffer cannot be allocated.  Otherwise each
+ * item's `status` is what pngb200_deflator_push would return.  Costs per call, whatever `count`: one upload of the new
+ * input, at most one deflate_resume_kernel launch over the items that compress, and one synchronise; an item that only
+ * enqueues costs its copy.  A CUDA error after the launch makes the error of the handles in it sticky. */
+typedef struct pngb200_deflator_push_desc {
+    pngb200_deflator* deflator;
+    const uint8_t*    data;      /* host memory, copied */
+    size_t            n;
+    int32_t           last;
+    int32_t           status;    /* out */
+} pngb200_deflator_push_desc;
+int    pngb200_deflator_push_batch(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t count);
+/* online handles: out[0] input bytes the device has dequeued (each byte once), out[1] compressed bytes written (the
+ * stream header included), out[2] blocks written, out[3] device bytes the handle holds now.  PNGB200_ERR_BAD_ARGUMENT
+ * for a buffered handle. */
+int    pngb200_deflator_stats(const pngb200_deflator* z, uint64_t out[4]);
 /* pop() : a complete block (exactly chunk_bytes) -> returns 1 and sets *block / *n (valid until the next call on
  * this handle); 0 = nil */
 int    pngb200_deflator_pop(pngb200_deflator* z, const uint8_t** block, size_t* n);

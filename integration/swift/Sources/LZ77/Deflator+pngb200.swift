@@ -17,7 +17,9 @@ extension LZ77
                 // a complete block is 2 * capacity bytes, capacity = what malloc grants for `hint` UInt16 atoms
                 // (LZ77.DeflatorOut.swift:15-27): 65544 for the encoder's hint of 1 << 15; 0 selects that value
                 let chunk:Int = hint == 1 << 15 ? 0 : 2 * hint
-                self.z = pngb200_deflator_create(LZ77.GPU.shared.ctx, format, Int32.init(level), Int32.init(exponent), chunk)!
+                // the online handle compresses as the pushes arrive, so pop() hands PNG.Encoder.pull each IDAT chunk
+                // when the reference would
+                self.z = pngb200_deflator_create_online(LZ77.GPU.shared.ctx, format, Int32.init(level), Int32.init(exponent), chunk)!
             }
             deinit
             {

@@ -178,6 +178,11 @@ class PngContextDesc(C.Structure):
     ]
 
 
+class DeflatorPushDesc(C.Structure):
+    _fields_ = [("deflator", C.c_void_p), ("data", C.c_void_p), ("n", C.c_size_t), ("last", C.c_int32),
+                ("status", C.c_int32)]
+
+
 class InflatorPushDesc(C.Structure):
     _fields_ = [("inflator", C.c_void_p), ("data", C.c_void_p), ("n", C.c_size_t), ("status", C.c_int32)]
 
@@ -253,6 +258,13 @@ def lib():
     L.pngb200_ctx_inflate_stats.restype = C.c_int
     L.pngb200_deflator_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_size_t]
     L.pngb200_deflator_create.restype = C.c_void_p
+    if os.environ.get("PNGB200_LIB") is None or hasattr(L, "pngb200_deflator_create_online"):   # (older builds lack it)
+        L.pngb200_deflator_create_online.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_size_t]
+        L.pngb200_deflator_create_online.restype = C.c_void_p
+        L.pngb200_deflator_push_batch.argtypes = [C.c_void_p, C.POINTER(DeflatorPushDesc), C.c_size_t]
+        L.pngb200_deflator_push_batch.restype = C.c_int
+        L.pngb200_deflator_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.pngb200_deflator_stats.restype = C.c_int
     L.pngb200_deflator_destroy.argtypes = [C.c_void_p]
     L.pngb200_deflator_destroy.restype = None
     L.pngb200_deflator_push.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.c_int]
@@ -827,14 +839,18 @@ def encode_batch(ctx: Context, images, level: int = 9):
 
 
 class Deflator:
-    """LZ77.Deflator value semantics (push(_:last:), pop(), pull()) over the GPU encoder."""
+    """LZ77.Deflator value semantics (push(_:last:), pop(), pull()) over the GPU encoder.  `online`: compress on the
+    device as the pushes arrive, so pop() hands out each block when the reference would (pngb200_deflator_create_online);
+    otherwise the whole stream is compressed at push(last: True)."""
 
-    def __init__(self, ctx: Context, fmt: int = FORMAT_ZLIB, level: int = 9, exponent: int = 15, chunk_bytes: int = 0):
+    def __init__(self, ctx: Context, fmt: int = FORMAT_ZLIB, level: int = 9, exponent: int = 15, chunk_bytes: int = 0,
+                 online: bool = False):
         self.ctx = ctx
         L = ctx._lib
-        self.handle = L.pngb200_deflator_create(ctx.handle, fmt, level, exponent, chunk_bytes)
+        create = L.pngb200_deflator_create_online if online else L.pngb200_deflator_create
+        self.handle = create(ctx.handle, fmt, level, exponent, chunk_bytes)
         if not self.handle:
-            raise PNGB200Error(ERR_BAD_ARGUMENT, "deflator_create")
+            raise PNGB200Error(ERR_BAD_ARGUMENT, L.pngb200_last_error(ctx.handle).decode())
 
     def close(self):
         if getattr(self, "handle", None):
@@ -860,6 +876,12 @@ class Deflator:
     def pull(self):
         """a complete block, else the flushed rest, else None (Swift: pull() -> [UInt8]?)"""
         return self._take(self.ctx._lib.pngb200_deflator_pull)
+
+    def stats(self) -> tuple:
+        """online handles: (input bytes dequeued, compressed bytes written, blocks written, device bytes held)"""
+        out = (C.c_uint64 * 4)()
+        self.ctx.check(self.ctx._lib.pngb200_deflator_stats(self.handle, out))
+        return tuple(out)
 
 
 class Inflator:
@@ -993,6 +1015,8 @@ def _push_batch(ctx: Context, kind, entry, items):
         d.n = len(data)
         if kind is PngPushDesc:
             d.overdraw = int(item[2])
+        elif kind is DeflatorPushDesc:
+            d.last = int(item[2])
     ctx.check(entry(ctx.handle, descs, len(items)))
     return [descs[i].status for i in range(len(items))]
 
@@ -1002,6 +1026,13 @@ def inflator_push_batch(ctx: Context, items) -> list:
     each push's status, as Inflator.push would return or raise it (payloads through the inflator's error()); raises
     PNGB200Error only when the call itself fails."""
     return _push_batch(ctx, InflatorPushDesc, ctx._lib.pngb200_inflator_push_batch, items)
+
+
+def deflator_push_batch(ctx: Context, items) -> list:
+    """push(_:last:) of many online Deflators in one call: `items` is [(deflator, data, last)], distinct online
+    deflators of `ctx`.  Returns each push's status, as Deflator.push would raise it; raises PNGB200Error only when the
+    call itself fails."""
+    return _push_batch(ctx, DeflatorPushDesc, ctx._lib.pngb200_deflator_push_batch, items)
 
 
 def png_context_push_batch(ctx: Context, items) -> list:

@@ -370,14 +370,16 @@ __device__ void df_store_vertex(DfState& z, uint8_t lit)
     z.count += 1;
 }
 
-// Stream.compress(all: true); returns true when the match buffer is full
-__device__ bool df_compress(DfState& z, DfShared& S)
+// Stream.compress(all:), Stream.swift:195-404; returns true when the match buffer is full.  `lookahead` is 0 for
+// compress(all: true), else 258 (greedy, full) or 259 (lazy): a head is taken only while more input than that is
+// pending (:210, :269, :345), so a key and a 258-byte compare never reach past z.n, and only all: true runs the epilogue.
+__device__ bool df_compress(DfState& z, DfShared& S, int64_t lookahead)
 {
     const unsigned lane = lane_id();
-    while (z.end_index < 0 && df_input_count(z) > 0) { z.end_index += 1; z.dequeued += 1; }
+    while (z.end_index < 0 && df_input_count(z) > lookahead) { z.end_index += 1; z.dequeued += 1; }
     int64_t next;
     if (z.mode == 0) {
-        while (df_input_count(z) > 0) {
+        while (df_input_count(z) > lookahead) {
             if (df_unfilled(z) <= 0) return true;
             int64_t a = df_window_update(z, &next);
             int run, dist;
@@ -388,7 +390,7 @@ __device__ bool df_compress(DfState& z, DfShared& S)
             z.count += 1;
         }
     } else if (z.mode == 1) {
-        while (df_input_count(z) > 0) {
+        while (df_input_count(z) > lookahead) {
             if (df_unfilled(z) <= 1) return true;
             int64_t a = df_window_update(z, &next);
             uint8_t first = df_literal(z, a);
@@ -418,12 +420,17 @@ __device__ bool df_compress(DfState& z, DfShared& S)
         // of the dictionary state at that position, so a batch does: (D) all 32 dictionary look-ups
         // against the pre-batch state in parallel, in-batch predecessors by warp match, one batched
         // update; (M) 32 independent chain walks; (S) the order-dependent skip rule over the lanes.
+        // A position is taken as a head while more than `lookahead` bytes are pending, and as a skip vertex of a long
+        // match whatever is pending (:376): `take` positions from a0 on qualify before this batch sets skip_until.
         uint32_t* g = z.graph;
-        while (df_input_count(z) > 0) {
+        for (;;) {
+            const int64_t a0 = z.end_index, left = df_input_count(z);
+            int64_t take = left - lookahead > z.skip_until - a0 ? left - lookahead : z.skip_until - a0;
+            if (take > left) take = left;
+            if (take <= 0) break;
             const int64_t unf = df_unfilled(z);
             if (unf <= 0) return true;
-            const int64_t a0 = z.end_index, left = df_input_count(z);
-            const int     nb = (int)(unf < 32 ? (unf < left ? unf : left) : (left < 32 ? left : 32));
+            const int     nb = (int)(unf < 32 ? (unf < take ? unf : take) : (take < 32 ? take : 32));
             const bool    act = (int)lane < nb;
             const int64_t a = a0 + lane;
             // ---- (D) ----
@@ -497,6 +504,7 @@ __device__ bool df_compress(DfState& z, DfShared& S)
             z.dequeued += nb;
         }
     }
+    if (lookahead > 0) return false;
     int64_t epilogue = -3 - (z.end_index < 0 ? z.end_index : 0);
     while (df_input_count(z) > epilogue) {
         if (df_unfilled(z) <= 0) return true;
@@ -798,6 +806,41 @@ __device__ int df_write_block(DfState& z, DfShared& S, DfOut& out, bool final)
     return 0;
 }
 
+// DeflatorSearch.init(level:) and the match buffer's capacity
+__device__ void df_search(DfState& z, int level)
+{
+    const int lv = level <= 0 ? 0 : level;
+    const long AT[13] = {1, 2, 4, 40, 20, 40, 64, 100, 14, 20, 30, 60, 100};
+    const int  GO[13] = {6, 8, 10, 24, 32, 54, 80, 160, 20, 32, 50, 80, 133};
+    if (lv <= 12) { z.mode = lv <= 3 ? 0 : lv <= 7 ? 1 : 2; z.attempts = AT[lv]; z.goal = GO[lv]; z.iterations = lv >= 8 ? lv - 7 : 0; }
+    else { z.mode = 2; z.attempts = 0x7fffffffffffffffL; z.goal = 258; z.iterations = 6; }
+    z.capacity = z.mode == 2 ? (int64_t)DF_GRAPH_CAP : (1 << 15);
+}
+
+// Depths.default into S.dflt, and into S.depths when `reset`
+__device__ void df_default_depths(DfShared& S, bool reset)
+{
+    for (uint32_t i = lane_id(); i < 542; i += 32) {
+        uint8_t v;
+        if (i < 256) v = 33;
+        else if (i < 512) { uint32_t run = i - 253; v = (uint8_t)(30 + (c_len_extra[df_run_decade(run) - 1] << 2)); }
+        else v = (uint8_t)(19 + (c_dist_extra[i - 512] << 2));
+        S.dflt[i] = v;
+        if (reset) S.depths[i] = v;
+    }
+    __syncwarp();
+}
+
+// the stored final block of a stream shorter than 3 bytes, Stream.swift:45-60, :417-435
+__device__ void df_write_stored(DfOut& out, const uint8_t* x, int64_t n)
+{
+    out.put(1, 3);
+    out.pad();
+    out.put((uint32_t)n, 16);
+    out.put(~(uint32_t)n & 0xffff, 16);
+    for (int64_t i = 0; i < n; ++i) out.put(x[i], 8);
+}
+
 __global__ void __launch_bounds__(32) deflate_kernel(DfParams P)
 {
     PNGB200_DYN_SMEM(df_smem);
@@ -821,28 +864,12 @@ __global__ void __launch_bounds__(32) deflate_kernel(DfParams P)
         z.next  = z.prevh + 32768;
         z.graph = reinterpret_cast<uint32_t*>(z.next + 32768);
         z.up    = z.graph + 32 * P.graph_vertices;
-        {   // DeflatorSearch.init(level:)
-            const int lv = job.level <= 0 ? 0 : job.level;
-            const long AT[13] = {1, 2, 4, 40, 20, 40, 64, 100, 14, 20, 30, 60, 100};
-            const int  GO[13] = {6, 8, 10, 24, 32, 54, 80, 160, 20, 32, 50, 80, 133};
-            if (lv <= 12) { z.mode = lv <= 3 ? 0 : lv <= 7 ? 1 : 2; z.attempts = AT[lv]; z.goal = GO[lv]; z.iterations = lv >= 8 ? lv - 7 : 0; }
-            else { z.mode = 2; z.attempts = 0x7fffffffffffffffL; z.goal = 258; z.iterations = 6; }
-        }
-        z.capacity = z.mode == 2 ? (int64_t)DF_GRAPH_CAP : (1 << 15);
+        df_search(z, job.level);
         int status = PNGB200_OK;
         if (z.mode == 2 && (uint64_t)(z.n < (int64_t)DF_GRAPH_CAP ? z.n : (int64_t)DF_GRAPH_CAP) + 2 > P.graph_vertices)
             status = PNGB200_ERR_INTERNAL;
         for (uint32_t i = lane; i < (1u << DF_HASH_BITS); i += 32) z.head[i] = -1;
-        // Depths.default
-        for (uint32_t i = lane; i < 542; i += 32) {
-            uint8_t v;
-            if (i < 256) v = 33;
-            else if (i < 512) { uint32_t run = i - 253; v = (uint8_t)(30 + (c_len_extra[df_run_decade(run) - 1] << 2)); }
-            else v = (uint8_t)(19 + (c_dist_extra[i - 512] << 2));
-            S.dflt[i] = v;
-            S.depths[i] = v;
-        }
-        __syncwarp();
+        df_default_depths(S, true);
         DfOut out;
         out.p = job.dst; out.cap = job.cap; out.bytes = 0; out.acc = 0; out.nacc = 0; out.overflow = 0;
         uint32_t blocks = 0;
@@ -856,18 +883,14 @@ __global__ void __launch_bounds__(32) deflate_kernel(DfParams P)
             }
             if (z.n >= 3) {
                 for (;;) {
-                    bool full = df_compress(z, S);
+                    bool full = df_compress(z, S, 0);
                     int rc = df_write_block(z, S, out, !full);
                     ++blocks;
                     if (rc) { status = rc; break; }
                     if (!full) break;
                 }
             } else {
-                out.put(1, 3);
-                out.pad();
-                out.put((uint32_t)z.n, 16);
-                out.put(~(uint32_t)z.n & 0xffff, 16);
-                for (int64_t i = 0; i < z.n; ++i) out.put(z.x[i], 8);
+                df_write_stored(out, z.x, z.n);
                 ++blocks;
             }
         }
@@ -902,6 +925,192 @@ __global__ void __launch_bounds__(32) deflate_kernel(DfParams P)
             res->produced = out.bytes;
             res->checksum = checksum;
             res->blocks = blocks;
+        }
+        __syncwarp();
+    }
+}
+
+// ---- the online deflator (pngb200_deflator_create_online): one launch per push batch, one warp per handle ----
+//
+// LZ77.DeflatorBuffers.push(_:last:) compresses whenever more than 4096 bytes are pending or `last` is set
+// (DeflatorBuffers.swift:68-137): compressBlocks(final: false) writes every block that fills while more input than the
+// lookahead is pending, and leaves the rest for a later push.  Everything that push carries lives in DfCarry and the
+// handle's device buffers.  Positions are relative to `base`, the absolute stream position of the handle's input byte 0;
+// after each non-final launch the base moves forward by a multiple of 32 768 (the dictionary slots `pos & mask` stay
+// put), so no position exceeds the unfinished block + the window + the pending input whatever the stream length.
+struct DfCarry {
+    int64_t  end_index, count, limit, skip_until;   // relative to base
+    uint64_t base;                                  // absolute position of input byte 0
+    uint64_t summed;                                // input bytes folded into the checksum (absolute)
+    uint64_t acc;                                   // the bit writer's partial byte
+    int32_t  nacc, generic, fresh, status;
+    uint32_t s1, s2, crc, pad;                      // running Adler-32 (s1, s2) and CRC-32
+    uint8_t  depths[544];                           // Depths carried across blocks (542 used)
+    uint32_t terms[2048];                           // greedy / lazy: the unfinished block's terms
+};
+struct DfResumeJob {
+    DfCarry*  carry;
+    uint8_t*  in;              // input from `base` on: n bytes
+    uint64_t  n;
+    int32_t*  dict;            // head, prevh, next
+    uint32_t* graph;           // full mode: the unfinished block's vertices, 32 words each
+    uint32_t* up;              // full mode: graph_vertices + 1 words, not carried
+    uint64_t  graph_vertices;
+    uint8_t*  dst;             // device: this launch's complete bytes, up to cap
+    uint64_t  cap;
+    uint8_t*  host_dst;        // where the warp copies them (pinned host memory)
+    struct DfResumeResult* result;   // pinned host memory
+    int32_t   format, level, exponent, last;
+};
+struct DfResumeResult {
+    int32_t  status;
+    uint32_t blocks;           // blocks written by this launch
+    uint64_t produced;         // complete bytes written by this launch
+    uint64_t base;             // the carry's base after it
+    int64_t  end_index, count; // relative to that base
+};
+// the carry of a handle that has compressed nothing yet
+inline void df_carry_init(DfCarry& c)
+{
+    memset(&c, 0, sizeof c);
+    c.end_index = -3;
+    c.limit = 2048;   // DeflatorMatches.init ignores its `limit:` argument
+    c.generic = 1;
+    c.fresh = 1;
+    c.s1 = 1;
+    c.crc = 0xffffffffu;
+}
+constexpr size_t DF_DICT_WORDS = (1u << DF_HASH_BITS) + 2 * 32768;
+
+__global__ void __launch_bounds__(32) deflate_resume_kernel(const DfResumeJob* jobs, int count)
+{
+    PNGB200_DYN_SMEM(df_smem);
+    DfShared& S = *reinterpret_cast<DfShared*>(df_smem);
+    const unsigned lane = lane_id();
+    for (int t = blockIdx.x; t < count; t += gridDim.x) {
+        const DfResumeJob job = jobs[t];
+        DfCarry&          c = *job.carry;
+        DfState z;
+        z.x = job.in; z.n = (int64_t)job.n;
+        const int exponent = job.format == PNGB200_FORMAT_IOS ? 15 : job.exponent;
+        z.mask = ((int64_t)1 << exponent) - 1;
+        z.end_index = c.end_index; z.dequeued = c.end_index + 3;   // the window has dequeued 3 bytes past its end
+        z.count = c.count; z.limit = c.limit; z.skip_until = c.skip_until; z.generic = c.generic;
+        z.head  = job.dict;
+        z.prevh = z.head + (1 << DF_HASH_BITS);
+        z.next  = z.prevh + 32768;
+        z.graph = job.graph;
+        z.up    = job.up;
+        df_search(z, job.level);
+        const bool fresh = c.fresh != 0;
+        if (fresh)
+            for (uint32_t i = lane; i < (1u << DF_HASH_BITS); i += 32) z.head[i] = -1;
+        df_default_depths(S, fresh);
+        if (!fresh)
+            for (uint32_t i = lane; i < 542; i += 32) S.depths[i] = c.depths[i];
+        if (z.mode != 2)
+            for (int64_t i = lane; i < z.count; i += 32) S.terms[i] = c.terms[i];
+        __syncwarp();
+        int status = c.status;
+        if (z.mode == 2 && (uint64_t)(z.count + (z.n - z.end_index)) + 2 > job.graph_vertices &&
+            (uint64_t)DF_GRAPH_CAP + 2 > job.graph_vertices)
+            status = PNGB200_ERR_INTERNAL;
+        // fold the bytes that arrived since the last launch into the checksum
+        uint32_t s1 = c.s1, s2 = c.s2, crc = c.crc;
+        const int64_t from = (int64_t)(c.summed - c.base);
+        if (job.format == PNGB200_FORMAT_ZLIB) {
+            for (int64_t b0 = from; b0 < z.n; b0 += 32 * 4096) {
+                const int64_t len = z.n - b0 < 32 * 4096 ? z.n - b0 : 32 * 4096;
+                uint64_t a = 0, b = 0;
+                for (int64_t k = lane; k < len; k += 32) { a += z.x[b0 + k]; b += (uint64_t)(len - k) * z.x[b0 + k]; }
+                for (int o = 16; o; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
+                s2 = (uint32_t)((s2 + (uint64_t)len % ADLER_MOD * s1 + b % ADLER_MOD) % ADLER_MOD);
+                s1 = (uint32_t)((s1 + a % ADLER_MOD) % ADLER_MOD);
+            }
+        } else if (job.format == PNGB200_FORMAT_GZIP) {
+            for (int64_t k = from; k < z.n; ++k) crc = crc32_byte_table((crc ^ z.x[k]) & 0xff) ^ (crc >> 8);
+        }
+        DfOut out;
+        out.p = job.dst; out.cap = job.cap; out.bytes = 0; out.acc = c.acc; out.nacc = c.nacc; out.overflow = 0;
+        uint32_t blocks = 0;
+        if (status == PNGB200_OK) {
+            const uint64_t total = c.base + (uint64_t)z.n;
+            if (job.last && total < 3) {
+                df_write_stored(out, z.x, z.n);   // never compacted: a stream this short has base 0
+                ++blocks;
+            } else {
+                const int64_t lookahead = job.last ? 0 : z.mode == 1 ? 259 : 258;
+                for (;;) {
+                    const bool full = df_compress(z, S, lookahead);
+                    if (!full && !job.last) break;
+                    const int rc = df_write_block(z, S, out, !full);
+                    ++blocks;
+                    if (rc) { status = rc; break; }
+                    if (!full) break;
+                }
+            }
+            if (job.last && job.format == PNGB200_FORMAT_ZLIB) {
+                const uint32_t ck = s2 << 16 | s1;
+                out.pad();
+                out.put(ck >> 24, 8); out.put((ck >> 16) & 0xff, 8); out.put((ck >> 8) & 0xff, 8); out.put(ck & 0xff, 8);
+            } else if (job.last && job.format == PNGB200_FORMAT_GZIP) {
+                const uint32_t ck = ~crc;
+                out.pad();
+                out.put(ck & 0xffff, 16); out.put(ck >> 16, 16);
+                out.put((uint32_t)total & 0xffff, 16); out.put(((uint32_t)total >> 16) & 0xffff, 16);
+            }
+            if (job.last) out.pad();
+            if (out.overflow) status = PNGB200_ERR_OUTPUT_CAPACITY;
+        }
+        // Move the base past what no later push reads: window look-ups and compares reach back to end_index - mask, and
+        // full mode reads the unfinished block's literals from end_index - count.
+        int64_t shift = 0;
+        if (status == PNGB200_OK && !job.last) {
+            int64_t keep = z.end_index - z.mask;
+            if (z.mode == 2 && z.end_index - z.count < keep) keep = z.end_index - z.count;
+            shift = keep > 0 ? keep >> 15 << 15 : 0;
+        }
+        if (shift) {
+            // positions that fall out of the window become -1, which ends a chain walk exactly as expiry does
+            uint4* d = reinterpret_cast<uint4*>(z.head);
+            const int32_t sh = (int32_t)shift;
+            auto rebase = [sh](uint32_t w) { return (int32_t)w >= sh ? (uint32_t)((int32_t)w - sh) : 0xffffffffu; };
+            for (uint32_t i = lane; i < DF_DICT_WORDS / 4; i += 32) {
+                uint4 v = d[i];
+                v.x = rebase(v.x); v.y = rebase(v.y); v.z = rebase(v.z); v.w = rebase(v.w);
+                d[i] = v;
+            }
+            // slide the live input down; a step moves 512 bytes, less than the shift, so a step reads nothing an
+            // earlier step wrote
+            const int64_t live = z.n - shift, vec = live >> 4;
+            uint4* dv = reinterpret_cast<uint4*>(job.in);
+            const uint4* sv = reinterpret_cast<const uint4*>(job.in + shift);
+            for (int64_t i0 = 0; i0 < vec; i0 += 32) {
+                if (i0 + lane < vec) dv[i0 + lane] = sv[i0 + lane];
+                __syncwarp();
+            }
+            for (int64_t i = (vec << 4) + lane; i < live; i += 32) job.in[i] = job.in[i + shift];
+            z.end_index -= shift;
+            z.skip_until -= shift;
+        }
+        __syncwarp();
+        // the complete bytes to the host
+        for (uint64_t i = lane; i < out.bytes && i < job.cap; i += 32) job.host_dst[i] = job.dst[i];
+        if (z.mode != 2)
+            for (int64_t i = lane; i < z.count; i += 32) c.terms[i] = S.terms[i];
+        for (uint32_t i = lane; i < 542; i += 32) c.depths[i] = S.depths[i];
+        __syncwarp();
+        if (lane == 0) {
+            c.end_index = z.end_index; c.count = z.count; c.limit = z.limit; c.skip_until = z.skip_until;
+            c.generic = z.generic; c.fresh = 0; c.status = status;
+            c.base += (uint64_t)shift;
+            c.summed = c.base + (uint64_t)(z.n - shift);
+            c.acc = out.acc; c.nacc = out.nacc;
+            c.s1 = s1; c.s2 = s2; c.crc = crc;
+            DfResumeResult r;
+            r.status = status; r.blocks = blocks; r.produced = out.bytes < job.cap ? out.bytes : job.cap;
+            r.base = c.base; r.end_index = z.end_index; r.count = z.count;
+            *job.result = r;
         }
         __syncwarp();
     }

@@ -116,6 +116,7 @@ struct pngb200_ctx {
     // bases and partials, and the staged input, apart from the decode batch's so that they may run while one is pending
     DevBuf d_st, d_stbase, d_stpartial, d_stin;
     PinBuf h_st, h_stin;
+    PinBuf h_dfout;   // the online deflators' launch: the bytes each handle wrote and its result, written by the kernel
     uint64_t seg_streams = 0, seg_segments = 0, seg_fallbacks = 0;  // last batch: streams cut into segments, segments, rejected
     uint64_t split_stats[6] = {};      // last batch, streams cut in two: see pngb200_ctx_split_stats
     uint64_t scratch_stride = 0;       // layout of d_scratch the last inflate launch used
@@ -1032,7 +1033,7 @@ pngb200_ctx* pngb200_ctx_create(int device)
         {(const void*)deflate_kernel, sizeof(DfShared)},          {(const void*)inflate_parallel_kernel3, sizeof(ParShared)},
         {(const void*)inflate_parallel_kernel, sizeof(ParShared)}, {(const void*)inflate_wave_kernel, sizeof(WvShared)},
         {(const void*)unfilter_wave_kernel, WAVE_SMEM},           {(const void*)inflate_cells_kernel, sizeof(ClShared)},
-        {(const void*)unfilter_pass_kernel, WAVE_SMEM}};
+        {(const void*)unfilter_pass_kernel, WAVE_SMEM},           {(const void*)deflate_resume_kernel, sizeof(DfShared)}};
     for (const auto& [kernel, bytes] : opt_in)
         if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess) {
             set_error(nullptr, PNGB200_ERR_CUDA, "cannot opt in to %zu bytes of shared memory", bytes);
@@ -1481,7 +1482,32 @@ int pngb200_filter_batch(pngb200_ctx* ctx, pngb200_filter_desc* im, size_t count
 
 }  // extern "C"
 
+namespace {
+
+// The call-level checks of the batch pushes: distinct handles of `ctx`, and data for every byte announced
+template <typename Desc, typename Handle>
+int check_pushes(pngb200_ctx* ctx, const Desc* pushes, size_t count, Handle* Desc::*handle, const char* what)
+{
+    if (!ctx || (!pushes && count)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "%s: null argument", what);
+    std::vector<const void*> seen(count);
+    for (size_t i = 0; i < count; ++i) {
+        const Handle* h = pushes[i].*handle;
+        if (!h || h->ctx != ctx || (!pushes[i].data && pushes[i].n))
+            return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "%s: item %zu has no handle of this context or no data", what, i);
+        seen[i] = h;
+    }
+    std::sort(seen.begin(), seen.end());
+    if (std::adjacent_find(seen.begin(), seen.end()) != seen.end())
+        return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "%s: a handle appears twice", what);
+    return PNGB200_OK;
+}
+
+}  // namespace
+
 // ---------------- streaming LZ77.Deflator handle ----------------
+// Two kinds: the buffered handle (pngb200_deflator_create) keeps the input on the host and compresses it in one
+// pngb200_deflate_batch call at push(last: true); the online handle (pngb200_deflator_create_online) compresses on the
+// device whenever the reference would, through deflate_resume_kernel, and keeps its state there between pushes.
 struct pngb200_deflator {
     pngb200_ctx*         ctx = nullptr;
     int                  format = 0, level = 9, exponent = 15;
@@ -1489,6 +1515,16 @@ struct pngb200_deflator {
     std::vector<uint8_t> input, output;
     size_t               at = 0;       // next output byte to hand out
     bool                 finished = false;
+    // online handles
+    bool     online = false;
+    int      status = PNGB200_OK;      // sticky: a failed launch leaves the device state unknown
+    DevBuf   d_carry, d_dict, d_graph, d_up, d_in, d_out;
+    uint64_t total = 0;                // bytes pushed
+    uint64_t base = 0;                 // stream position of d_in's byte 0
+    int64_t  end_index = -3, count = 0;   // the carry's window end (relative to base) and match-buffer fill
+    uint64_t blocks = 0, written = 0;   // blocks and bytes written, the stream header included
+    uint64_t dequeued() const { return std::min<uint64_t>(total, (uint64_t)std::max<int64_t>(0, (int64_t)base + end_index + 3)); }
+    size_t   device_bytes() const { return d_carry.cap + d_dict.cap + d_graph.cap + d_up.cap + d_in.cap + d_out.cap; }
 };
 
 extern "C" {
@@ -1508,11 +1544,224 @@ pngb200_deflator* pngb200_deflator_create(pngb200_ctx* ctx, int format, int leve
     return z;
 }
 
-void pngb200_deflator_destroy(pngb200_deflator* z) { delete z; }
+pngb200_deflator* pngb200_deflator_create_online(pngb200_ctx* ctx, int format, int level, int exponent, size_t chunk_bytes)
+{
+    pngb200_deflator* z = pngb200_deflator_create(ctx, format, level, exponent, chunk_bytes);
+    if (!z) return nullptr;
+    z->online = true;
+    DeviceGuard guard(ctx->device);
+    DfCarry init;
+    df_carry_init(init);
+    if (z->d_carry.reserve(sizeof(DfCarry)) != cudaSuccess || z->d_dict.reserve(sizeof(int32_t) * DF_DICT_WORDS) != cudaSuccess ||
+        cudaMemcpy(z->d_carry.p, &init, sizeof init, cudaMemcpyHostToDevice) != cudaSuccess) {
+        set_error(ctx, PNGB200_ERR_CUDA, "deflator_create_online: cannot allocate the device state");
+        delete z;
+        return nullptr;
+    }
+    // DeflatorBuffers.init writes the stream header (DeflatorBuffers.swift:50-65, Gzip :100-112)
+    const int e = format == PNGB200_FORMAT_IOS ? 15 : exponent;
+    if (format == PNGB200_FORMAT_ZLIB) {
+        const uint32_t unpaired = (uint32_t)(e - 8) << 4 | 8, check = ~(((unpaired << 8) | (unpaired >> 8)) % 31) & 31;
+        z->output = {(uint8_t)unpaired, (uint8_t)check};
+    } else if (format == PNGB200_FORMAT_GZIP) {
+        z->output = {0x1f, 0x8b, 0x08, 0x00, 0x00, 0x00, 0x00, 0x00, 0x00, 0xff};
+    }
+    z->written = z->output.size();
+    return z;
+}
+
+void pngb200_deflator_destroy(pngb200_deflator* z)
+{
+    if (!z) return;
+    if (z->online) {
+        DeviceGuard guard(z->ctx->device);
+        cudaStreamSynchronize(z->ctx->stream);
+    }
+    delete z;   // frees the device state
+}
+
+}  // extern "C"
+
+namespace {
+
+// The pushes of one pngb200_deflator_push_batch call, on distinct online handles of `ctx`.  Every buffer the call
+// needs is allocated before any device work, so that an allocation failure leaves every handle as it was.
+int deflator_pushes(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t count)
+{
+    constexpr uint64_t kMaxPush = 1ull << 30;   // keeps every position of a launch inside int32
+    std::vector<pngb200_deflator_push_desc*> live;
+    size_t staged = 0;
+    for (size_t i = 0; i < count; ++i) {
+        pngb200_deflator_push_desc* d = &pushes[i];
+        pngb200_deflator* z = d->deflator;
+        if (z->status < 0) d->status = z->status;
+        else if (z->finished) d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "deflator: push after push(last: true)");
+        else if (d->n > kMaxPush) d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "deflator: a push is at most 1 GiB");
+        else live.push_back(d), staged += d->n;
+    }
+    // What each live item needs: input from the base on; when it compresses, a graph for every vertex the push can add
+    // to the unfinished block (full mode) and room for every byte the launch can write.
+    struct Need { bool run; size_t in, graph, up, out; };
+    std::vector<Need> need(live.size());
+    size_t run = 0, host_out = 0;
+    for (size_t k = 0; k < live.size(); ++k) {
+        const pngb200_deflator* z = live[k]->deflator;
+        const uint64_t total = z->total + live[k]->n, n = total - z->base;
+        const uint64_t pending = total - z->dequeued();
+        Need& w = need[k];
+        w.run = pending > 4096 || live[k]->last;   // DeflatorBuffers.swift:74, :120
+        w.in = n + 16;
+        w.graph = w.up = w.out = 0;
+        if (w.run) {
+            const bool full = z->level >= 8;
+            const uint64_t span = (uint64_t)((int64_t)n - z->end_index);
+            const uint64_t verts = std::min<uint64_t>(DF_GRAPH_CAP, (uint64_t)z->count + span) + 2;
+            if (full) w.graph = 128 * verts, w.up = 4 * (verts + 1);
+            w.out = pngb200_deflate_bound((full ? 1 : 8) * (uint64_t)z->count + span) + 4096;
+            host_out += align_up(w.out, 256);
+            run++;
+        }
+    }
+    // allocations
+    std::vector<DevBuf> grown_in(live.size()), grown_graph(live.size());
+    CU(ctx->h_stin.reserve(std::max<size_t>(staged, 1)));
+    CU(ctx->d_stin.reserve(std::max<size_t>(staged, 1)));
+    const size_t jobs_bytes = sizeof(DfResumeJob) * std::max<size_t>(run, 1);
+    const size_t res_off = align_up(host_out, 256);
+    CU(ctx->h_dfout.reserve(res_off + sizeof(DfResumeResult) * std::max<size_t>(run, 1)));
+    CU(ctx->h_st.reserve(jobs_bytes));
+    CU(ctx->d_st.reserve(jobs_bytes));
+    for (size_t k = 0; k < live.size(); ++k) {
+        pngb200_deflator* z = live[k]->deflator;
+        if (need[k].in > z->d_in.cap) CU(grown_in[k].reserve(need[k].in));
+        if (need[k].graph > z->d_graph.cap) CU(grown_graph[k].reserve(need[k].graph));
+        CU(z->d_up.reserve(need[k].up));
+        CU(z->d_out.reserve(need[k].out));
+    }
+    // device work: the new input of every handle with one upload, then appended to each handle's input
+    for (pngb200_deflator_push_desc* d : live) d->status = PNGB200_ERR_CUDA;
+    std::vector<DevBuf> retired;
+    auto fail = [&](int rc) { cudaStreamSynchronize(ctx->stream); return rc; };
+    size_t off = 0;
+    for (pngb200_deflator_push_desc* d : live)
+        if (d->n) memcpy(ctx->h_stin.as<uint8_t>() + off, d->data, d->n), off += d->n;
+    if (staged && cudaMemcpyAsync(ctx->d_stin.p, ctx->h_stin.p, staged, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
+        return fail(set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: input upload failed"));
+    std::vector<DfResumeJob> jobs;
+    std::vector<size_t>      which;
+    off = 0;
+    size_t out_at = 0;
+    for (size_t k = 0; k < live.size(); ++k) {
+        pngb200_deflator_push_desc* d = live[k];
+        pngb200_deflator* z = d->deflator;
+        const size_t held = z->total - z->base;
+        if (grown_in[k].p) {
+            if (held && cudaMemcpyAsync(grown_in[k].p, z->d_in.p, held, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
+                return fail(set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: input copy failed"));
+            std::swap(z->d_in, grown_in[k]);
+        }
+        if (grown_graph[k].p) {
+            if (z->count && cudaMemcpyAsync(grown_graph[k].p, z->d_graph.p, 128 * (size_t)z->count, cudaMemcpyDeviceToDevice,
+                                            ctx->stream) != cudaSuccess)
+                return fail(set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: graph copy failed"));
+            std::swap(z->d_graph, grown_graph[k]);
+        }
+        if (d->n && cudaMemcpyAsync(z->d_in.as<uint8_t>() + held, ctx->d_stin.as<uint8_t>() + off, d->n,
+                                    cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
+            return fail(set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: input copy failed"));
+        off += d->n;
+        z->total += d->n;
+        // what the reference's pop() handed out is gone from the queue
+        z->output.erase(z->output.begin(), z->output.begin() + (ptrdiff_t)z->at);
+        z->at = 0;
+        if (!need[k].run) {
+            d->status = PNGB200_OK;
+            continue;
+        }
+        DfResumeJob j;
+        j.carry = z->d_carry.as<DfCarry>();
+        j.in = z->d_in.as<uint8_t>();
+        j.n = z->total - z->base;
+        j.dict = z->d_dict.as<int32_t>();
+        j.graph = z->d_graph.as<uint32_t>();
+        j.up = z->d_up.as<uint32_t>();
+        j.graph_vertices = z->d_graph.cap / 128;
+        j.dst = z->d_out.as<uint8_t>();
+        j.cap = need[k].out;
+        j.host_dst = ctx->h_dfout.as<uint8_t>() + out_at;   // pinned: the kernel writes it over the bus (unified addressing)
+        j.result = (DfResumeResult*)(ctx->h_dfout.as<uint8_t>() + res_off) + jobs.size();
+        j.format = z->format;
+        j.level = z->level;
+        j.exponent = z->exponent;
+        j.last = d->last ? 1 : 0;
+        out_at += align_up(need[k].out, 256);
+        jobs.push_back(j);
+        which.push_back(k);
+    }
+    if (!jobs.empty()) {
+        memcpy(ctx->h_st.p, jobs.data(), sizeof(DfResumeJob) * jobs.size());
+        cudaError_t e = cudaMemcpyAsync(ctx->d_st.p, ctx->h_st.p, sizeof(DfResumeJob) * jobs.size(), cudaMemcpyHostToDevice,
+                                        ctx->stream);
+        if (e == cudaSuccess) {
+            deflate_resume_kernel<<<(unsigned)jobs.size(), 32, sizeof(DfShared), ctx->stream>>>(ctx->d_st.as<DfResumeJob>(),
+                                                                                                 (int)jobs.size());
+            ctx->launches++;
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        for (size_t t = 0; t < jobs.size(); ++t) {
+            pngb200_deflator_push_desc* d = live[which[t]];
+            pngb200_deflator* z = d->deflator;
+            if (e != cudaSuccess) {
+                z->status = d->status = set_error(ctx, PNGB200_ERR_CUDA, "deflate_resume_kernel: %s", cudaGetErrorString(e));
+                continue;
+            }
+            const DfResumeResult& r = *jobs[t].result;
+            d->status = r.status;
+            if (r.status != PNGB200_OK) {
+                z->status = set_error(ctx, r.status, "deflate_resume_kernel: status %d", r.status);
+                continue;
+            }
+            z->output.insert(z->output.end(), jobs[t].host_dst, jobs[t].host_dst + r.produced);
+            z->blocks += r.blocks;
+            z->written += r.produced;
+            z->base = r.base;
+            z->end_index = r.end_index;
+            z->count = r.count;
+            if (d->last) z->finished = true;
+        }
+        if (e != cudaSuccess) return PNGB200_ERR_CUDA;
+    } else if (staged) {
+        if (cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+            return set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: synchronise failed");
+    }
+    return PNGB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pngb200_deflator_push_batch(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t count)
+{
+    if (int rc = check_pushes(ctx, pushes, count, &pngb200_deflator_push_desc::deflator, "deflator_push_batch")) return rc;
+    for (size_t i = 0; i < count; ++i)
+        if (!pushes[i].deflator->online)
+            return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "deflator_push_batch: item %zu is a buffered deflator", i);
+    if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a decode batch is pending");
+    if (!count) return PNGB200_OK;
+    DeviceGuard guard(ctx->device);
+    return deflator_pushes(ctx, pushes, count);
+}
 
 int pngb200_deflator_push(pngb200_deflator* z, const uint8_t* data, size_t n, int last)
 {
     if (!z || (!data && n)) return PNGB200_ERR_BAD_ARGUMENT;
+    if (z->online) {
+        pngb200_deflator_push_desc d{z, data, n, last, 0};
+        if (int rc = pngb200_deflator_push_batch(z->ctx, &d, 1)) return rc;
+        return d.status;
+    }
     if (z->finished) return set_error(z->ctx, PNGB200_ERR_BAD_ARGUMENT, "deflator: push after push(last: true)");
     z->input.insert(z->input.end(), data, data + n);
     if (!last) return PNGB200_OK;
@@ -1538,8 +1787,9 @@ int pngb200_deflator_push(pngb200_deflator* z, const uint8_t* data, size_t n, in
 int pngb200_deflator_pop(pngb200_deflator* z, const uint8_t** block, size_t* n)
 {
     if (!z || !block || !n) return PNGB200_ERR_BAD_ARGUMENT;
-    // DeflatorOut queues a block the moment its buffer is full (LZ77.DeflatorOut.swift:109-135): complete blocks only
-    if (!z->finished || z->output.size() - z->at < z->chunk) return 0;
+    // DeflatorOut queues a block the moment its buffer is full (LZ77.DeflatorOut.swift:109-135): complete blocks only.
+    // The buffered handle has none before push(last: true).
+    if ((!z->online && !z->finished) || z->output.size() - z->at < z->chunk) return 0;
     *block = z->output.data() + z->at;
     *n = z->chunk;
     z->at += z->chunk;
@@ -1555,6 +1805,16 @@ int pngb200_deflator_pull(pngb200_deflator* z, const uint8_t** block, size_t* n)
     *n = z->output.size() - z->at;
     z->at = z->output.size();
     return 1;
+}
+
+int pngb200_deflator_stats(const pngb200_deflator* z, uint64_t out[4])
+{
+    if (!z || !out || !z->online) return PNGB200_ERR_BAD_ARGUMENT;
+    out[0] = z->dequeued();
+    out[1] = z->written;
+    out[2] = z->blocks;
+    out[3] = z->device_bytes();
+    return PNGB200_OK;
 }
 
 }  // extern "C"
@@ -2032,24 +2292,6 @@ int inflate_pushes(pngb200_ctx* ctx, pngb200_inflator_push_desc* const* items, s
         }
         round.swap(again);
     }
-    return PNGB200_OK;
-}
-
-// The call-level checks of both batch pushes: distinct handles of `ctx`, and data for every byte announced
-template <typename Desc, typename Handle>
-int check_pushes(pngb200_ctx* ctx, const Desc* pushes, size_t count, Handle* Desc::*handle, const char* what)
-{
-    if (!ctx || (!pushes && count)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "%s: null argument", what);
-    std::vector<const void*> seen(count);
-    for (size_t i = 0; i < count; ++i) {
-        const Handle* h = pushes[i].*handle;
-        if (!h || h->ctx != ctx || (!pushes[i].data && pushes[i].n))
-            return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "%s: item %zu has no handle of this context or no data", what, i);
-        seen[i] = h;
-    }
-    std::sort(seen.begin(), seen.end());
-    if (std::adjacent_find(seen.begin(), seen.end()) != seen.end())
-        return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "%s: a handle appears twice", what);
     return PNGB200_OK;
 }
 
