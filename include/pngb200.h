@@ -106,8 +106,10 @@ typedef struct pngb200_ctx pngb200_ctx;
  * sm_90 device, out of memory); pngb200_last_error(NULL) then describes why. */
 pngb200_ctx* pngb200_ctx_create(int device);
 void         pngb200_ctx_destroy(pngb200_ctx* ctx);
-/* Return the context's grow-only device arenas (and its pipeline lanes') to the driver; the next
- * batch call allocates again.  Fails with BAD_ARGUMENT while a decode batch is pending. */
+/* Return the context's grow-only device arenas (and its pipeline lanes') to the driver, the streaming
+ * handles' push workspaces (tables, checksum partials, staged input and the pinned host buffers behind them)
+ * included; the next batch call or push allocates again.  The handles keep their own buffers.  Fails with
+ * BAD_ARGUMENT while a decode batch is pending. */
 int          pngb200_ctx_trim(pngb200_ctx* ctx);
 const char*  pngb200_last_error(const pngb200_ctx* ctx);
 /* the cudaStream_t all of this context's work is enqueued on (for event timing / interop) */
@@ -439,8 +441,10 @@ int    pngb200_inflator_stats(const pngb200_inflator* z, uint64_t out[3]);
  * have workspaces of their own).
  * Returns PNGB200_OK once every item's status is written, even when some items failed; PNGB200_ERR_BAD_ARGUMENT, before
  * any work and with no item touched, for a null ctx, pushes NULL with count > 0, a null handle, a handle of another ctx,
- * the same handle twice, or data NULL with n > 0 (count == 0 is OK); PNGB200_ERR_CUDA on a CUDA failure, each item not
- * finished then left as a single push failing the same way would leave it (status PNGB200_ERR_CUDA).
+ * the same handle twice, or data NULL with n > 0 (count == 0 is OK); PNGB200_ERR_CUDA, with every handle unchanged, when
+ * the staged input or a buffer a handle grows to take its push in cannot be allocated; PNGB200_ERR_CUDA on any other
+ * CUDA failure (a later allocation included), each item not finished then left as a single push failing the same way
+ * would leave it (status PNGB200_ERR_CUDA).
  * Fixed cost, whatever `count`: one round of at most 2 kernel launches (the ring inflate kernel over the items with
  * 64 KiB or more of undecoded input, the serial one over the rest) and 1 stream synchronise, then, when streams ended,
  * 2 checksum launches and 1 synchronise.  An item whose output buffer has to grow goes again in a further round, with

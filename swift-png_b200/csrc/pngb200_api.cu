@@ -219,6 +219,57 @@ struct Tables {
     template <typename T> T* pin(size_t off) const { return (T*)((char*)h.p + off); }
 };
 
+// The buffers one push call grows and the input it stages.  grow() takes the buffers add() listed in two phases.
+// Phase 1 allocates a replacement for each and room to stage `staged` pushed bytes; it touches no handle and enqueues
+// no device work, so a failure leaves every handle as it was.  Phase 2 copies each buffer's first `keep` bytes into
+// its replacement on the stream and swaps the replacement in.  The buffers replaced are freed with this object, after
+// the call's last synchronise: done() says the call ended in one; on any other way out the destructor makes it, since
+// the stream may still be reading them, the staging or the caller's memory.
+struct PushCall {
+    struct Grow { DevBuf* buf; size_t size, keep; DevBuf next; };
+    pngb200_ctx*        ctx;
+    std::vector<Grow>   list;
+    std::vector<DevBuf> replaced;
+    bool                synced = false;
+    explicit PushCall(pngb200_ctx* c) : ctx(c) {}
+    ~PushCall() { if (!synced) cudaStreamSynchronize(ctx->stream); }
+    void add(DevBuf& b, size_t size, size_t keep) { list.push_back({&b, size, keep, DevBuf()}); }
+    int grow(size_t staged)
+    {
+        CU(ctx->h_stin.reserve(staged));
+        CU(ctx->d_stin.reserve(staged));
+        for (Grow& g : list) CU(g.next.reserve(g.size));
+        for (Grow& g : list) {
+            if (g.keep) CU(cudaMemcpyAsync(g.next.p, g.buf->p, g.keep, cudaMemcpyDeviceToDevice, ctx->stream));
+            std::swap(*g.buf, g.next);
+            replaced.push_back(std::move(g.next));
+        }
+        list.clear();
+        return PNGB200_OK;
+    }
+    // Packs the items' bytes into the staging, uploads them with one copy and appends each item's at byte held() of
+    // its handle's d_in; `appended(d)` counts them in once that copy is queued.
+    template <typename Desc, typename Handle, typename Appended>
+    int stage(const std::vector<Desc*>& items, Handle* Desc::*handle, Appended appended)
+    {
+        size_t off = 0;
+        for (const Desc* d : items)
+            if (d->n) memcpy(ctx->h_stin.as<uint8_t>() + off, d->data, d->n), off += d->n;
+        if (off) CU(cudaMemcpyAsync(ctx->d_stin.p, ctx->h_stin.p, off, cudaMemcpyHostToDevice, ctx->stream));
+        off = 0;
+        for (Desc* d : items) {
+            Handle* z = d->*handle;
+            if (d->n)
+                CU(cudaMemcpyAsync((uint8_t*)z->d_in.p + z->held(), ctx->d_stin.as<uint8_t>() + off, d->n,
+                                   cudaMemcpyDeviceToDevice, ctx->stream));
+            off += d->n;
+            appended(d);
+        }
+        return PNGB200_OK;
+    }
+    int done() { synced = true; return PNGB200_OK; }
+};
+
 // the CRC-32 byte table and shift operators (crc32.cuh), uploaded once per context
 int ensure_crc_tables(pngb200_ctx* ctx)
 {
@@ -1068,8 +1119,10 @@ int pngb200_ctx_trim(pngb200_ctx* ctx)
     for (pngb200_ctx* lane : ctx->lanes) pngb200_ctx_trim(lane);
     DeviceGuard guard(ctx->device);
     CU(cudaStreamSynchronize(ctx->stream));
-    for (DevBuf* b : {&ctx->d_partial, &ctx->d_filtered, &ctx->d_in, &ctx->d_out, &ctx->d_scratch, &ctx->d_dfscratch, &ctx->d_enc, &ctx->d_file, &ctx->d_sgsym, &ctx->d_sgwin})
+    for (DevBuf* b : {&ctx->d_partial, &ctx->d_filtered, &ctx->d_in, &ctx->d_out, &ctx->d_scratch, &ctx->d_dfscratch, &ctx->d_enc, &ctx->d_file, &ctx->d_sgsym, &ctx->d_sgwin,
+                      &ctx->d_st, &ctx->d_stbase, &ctx->d_stpartial, &ctx->d_stin})
         b->release();
+    for (PinBuf* b : {&ctx->h_st, &ctx->h_stin, &ctx->h_dfout}) b->release();
     ctx->scratch_stride = 0;
     return PNGB200_OK;
 }
@@ -1523,6 +1576,7 @@ struct pngb200_deflator {
     uint64_t base = 0;                 // stream position of d_in's byte 0
     int64_t  end_index = -3, count = 0;   // the carry's window end (relative to base) and match-buffer fill
     uint64_t blocks = 0, written = 0;   // blocks and bytes written, the stream header included
+    uint64_t held() const { return total - base; }   // bytes of d_in in use
     uint64_t dequeued() const { return std::min<uint64_t>(total, (uint64_t)std::max<int64_t>(0, (int64_t)base + end_index + 3)); }
     size_t   device_bytes() const { return d_carry.cap + d_dict.cap + d_graph.cap + d_up.cap + d_in.cap + d_out.cap; }
 };
@@ -1597,7 +1651,7 @@ int deflator_pushes(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t
         if (z->status < 0) d->status = z->status;
         else if (z->finished) d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "deflator: push after push(last: true)");
         else if (d->n > kMaxPush) d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "deflator: a push is at most 1 GiB");
-        else live.push_back(d), staged += d->n;
+        else d->status = PNGB200_ERR_CUDA, live.push_back(d), staged += d->n;   // until its push is answered
     }
     // What each live item needs: input from the base on; when it compresses, a graph for every vertex the push can add
     // to the unfinished block (full mode) and room for every byte the launch can write.
@@ -1622,10 +1676,8 @@ int deflator_pushes(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t
             run++;
         }
     }
-    // allocations
-    std::vector<DevBuf> grown_in(live.size()), grown_graph(live.size());
-    CU(ctx->h_stin.reserve(std::max<size_t>(staged, 1)));
-    CU(ctx->d_stin.reserve(std::max<size_t>(staged, 1)));
+    // every allocation, before any device work
+    PushCall call(ctx);
     const size_t jobs_bytes = sizeof(DfResumeJob) * std::max<size_t>(run, 1);
     const size_t res_off = align_up(host_out, 256);
     CU(ctx->h_dfout.reserve(res_off + sizeof(DfResumeResult) * std::max<size_t>(run, 1)));
@@ -1633,44 +1685,22 @@ int deflator_pushes(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t
     CU(ctx->d_st.reserve(jobs_bytes));
     for (size_t k = 0; k < live.size(); ++k) {
         pngb200_deflator* z = live[k]->deflator;
-        if (need[k].in > z->d_in.cap) CU(grown_in[k].reserve(need[k].in));
-        if (need[k].graph > z->d_graph.cap) CU(grown_graph[k].reserve(need[k].graph));
-        CU(z->d_up.reserve(need[k].up));
-        CU(z->d_out.reserve(need[k].out));
+        if (need[k].in > z->d_in.cap) call.add(z->d_in, need[k].in, z->held());
+        if (need[k].graph > z->d_graph.cap) call.add(z->d_graph, need[k].graph, 128 * (size_t)z->count);
+        if (need[k].up > z->d_up.cap) call.add(z->d_up, need[k].up, 0);
+        if (need[k].out > z->d_out.cap) call.add(z->d_out, need[k].out, 0);
     }
-    // device work: the new input of every handle with one upload, then appended to each handle's input
-    for (pngb200_deflator_push_desc* d : live) d->status = PNGB200_ERR_CUDA;
-    std::vector<DevBuf> retired;
-    auto fail = [&](int rc) { cudaStreamSynchronize(ctx->stream); return rc; };
-    size_t off = 0;
-    for (pngb200_deflator_push_desc* d : live)
-        if (d->n) memcpy(ctx->h_stin.as<uint8_t>() + off, d->data, d->n), off += d->n;
-    if (staged && cudaMemcpyAsync(ctx->d_stin.p, ctx->h_stin.p, staged, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
-        return fail(set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: input upload failed"));
+    if (int rc = call.grow(staged)) return rc;
+    // the new input of every handle with one upload, appended to its input
+    if (int rc = call.stage(live, &pngb200_deflator_push_desc::deflator,
+                            [](pngb200_deflator_push_desc* d) { d->deflator->total += d->n; }))
+        return rc;
     std::vector<DfResumeJob> jobs;
     std::vector<size_t>      which;
-    off = 0;
     size_t out_at = 0;
     for (size_t k = 0; k < live.size(); ++k) {
         pngb200_deflator_push_desc* d = live[k];
         pngb200_deflator* z = d->deflator;
-        const size_t held = z->total - z->base;
-        if (grown_in[k].p) {
-            if (held && cudaMemcpyAsync(grown_in[k].p, z->d_in.p, held, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
-                return fail(set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: input copy failed"));
-            std::swap(z->d_in, grown_in[k]);
-        }
-        if (grown_graph[k].p) {
-            if (z->count && cudaMemcpyAsync(grown_graph[k].p, z->d_graph.p, 128 * (size_t)z->count, cudaMemcpyDeviceToDevice,
-                                            ctx->stream) != cudaSuccess)
-                return fail(set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: graph copy failed"));
-            std::swap(z->d_graph, grown_graph[k]);
-        }
-        if (d->n && cudaMemcpyAsync(z->d_in.as<uint8_t>() + held, ctx->d_stin.as<uint8_t>() + off, d->n,
-                                    cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess)
-            return fail(set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: input copy failed"));
-        off += d->n;
-        z->total += d->n;
         // what the reference's pop() handed out is gone from the queue
         z->output.erase(z->output.begin(), z->output.begin() + (ptrdiff_t)z->at);
         z->at = 0;
@@ -1735,7 +1765,7 @@ int deflator_pushes(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t
         if (cudaStreamSynchronize(ctx->stream) != cudaSuccess)
             return set_error(ctx, PNGB200_ERR_CUDA, "deflator_push_batch: synchronise failed");
     }
-    return PNGB200_OK;
+    return call.done();
 }
 
 }  // namespace
@@ -2099,9 +2129,9 @@ extern "C" {
 struct pngb200_inflator {
     pngb200_ctx*         ctx;
     int                  format;
-    std::vector<uint8_t> input;      // everything pushed so far
-    DevBuf               d_in, d_out;
-    size_t               uploaded = 0;
+    DevBuf               d_in, d_out;     // every byte pushed; the output
+    uint64_t             pushed = 0, tail_at = 0;
+    std::vector<uint8_t> tail;            // the input from byte tail_at <= resume_bit >> 3 on (stored_in_flight)
     uint64_t             resume_bit = 0, resume_out = 0, produced = 0, current = 0;
     uint32_t             phase = 0;
     ResumePoint          at{};            // the block a phase-3 resume point lies in (uploaded with every launch)
@@ -2109,6 +2139,7 @@ struct pngb200_inflator {
     bool                 terminal = false;
     int                  status = PNGB200_NEED_MORE_INPUT;
     uint32_t             err_a = 0, err_b = 0;
+    uint64_t             held() const { return pushed; }   // bytes of d_in in use
 };
 
 pngb200_inflator* pngb200_inflator_create(pngb200_ctx* ctx, int format)
@@ -2132,28 +2163,15 @@ void pngb200_inflator_destroy(pngb200_inflator* z)
 
 namespace {
 
-// Grows a device buffer to at least `need` bytes, carrying its first `keep` bytes over device to device.  The old
-// memory goes to `retired`, which the caller frees once the stream has passed the copy.
-int grow_carrying(pngb200_ctx* ctx, DevBuf& b, size_t need, size_t keep, std::vector<DevBuf>& retired)
-{
-    if (need <= b.cap) return PNGB200_OK;
-    DevBuf bigger;
-    CU(bigger.reserve(need));
-    if (keep) CU(cudaMemcpyAsync(bigger.p, b.p, keep, cudaMemcpyDeviceToDevice, ctx->stream));
-    std::swap(b, bigger);
-    retired.push_back(std::move(bigger));
-    return PNGB200_OK;
-}
-
 // The pushes of one pngb200_inflator_push_batch call, on distinct handles of `ctx`.  Every item's `status` is
 // PNGB200_ERR_CUDA until its push is answered, so that a CUDA failure leaves the items it stopped as a single push that
-// failed the same way.  `retired`: buffers the caller frees after its final stream synchronise.
-int inflate_pushes(pngb200_ctx* ctx, pngb200_inflator_push_desc* const* items, size_t count, std::vector<DevBuf>& retired)
+// failed the same way.
+int inflate_pushes(pngb200_ctx* ctx, pngb200_inflator_push_desc* pushes, size_t count)
 {
     std::vector<pngb200_inflator_push_desc*> live;
     size_t staged = 0;
     for (size_t i = 0; i < count; ++i) {
-        pngb200_inflator_push_desc* d = items[i];
+        pngb200_inflator_push_desc* d = &pushes[i];
         pngb200_inflator* z = d->inflator;
         if (z->terminal) d->status = PNGB200_OK;   // LZ77.Inflator ignores input after the terminal state
         else if (z->status < 0) d->status = z->status;
@@ -2164,30 +2182,26 @@ int inflate_pushes(pngb200_ctx* ctx, pngb200_inflator_push_desc* const* items, s
         }
     }
     if (live.empty()) return PNGB200_OK;
-    // the new input of every handle: one upload into staging, then appended to each handle's device copy
-    if (staged) {
-        CU(ctx->h_stin.reserve(staged));
-        CU(ctx->d_stin.reserve(staged));
-        size_t off = 0;
-        for (pngb200_inflator_push_desc* d : live)
-            if (d->n) memcpy(ctx->h_stin.as<uint8_t>() + off, d->data, d->n), off += d->n;
-        CU(cudaMemcpyAsync(ctx->d_stin.p, ctx->h_stin.p, staged, cudaMemcpyHostToDevice, ctx->stream));
-    }
-    size_t off = 0;
+    PushCall call(ctx);
     for (pngb200_inflator_push_desc* d : live) {
         pngb200_inflator* z = d->inflator;
-        z->input.insert(z->input.end(), d->data, d->data + d->n);
-        if (z->input.size() + 16 > z->d_in.cap)   // 16 bytes of slack behind the input for the decoders' bit reader
-            if (int rc = grow_carrying(ctx, z->d_in, z->input.size() * 2 + 4096, z->uploaded, retired)) return rc;
-        if (d->n)
-            CU(cudaMemcpyAsync(z->d_in.as<uint8_t>() + z->uploaded, ctx->d_stin.as<uint8_t>() + off, d->n,
-                               cudaMemcpyDeviceToDevice, ctx->stream));
-        off += d->n;
-        z->uploaded = z->input.size();
+        const uint64_t pushed = z->pushed + d->n;
+        if (pushed + 16 > z->d_in.cap)   // 16 bytes of slack behind the input for the decoders' bit reader
+            call.add(z->d_in, pushed * 2 + 4096, z->pushed);
         const size_t want = std::max<size_t>(1 << 16, z->produced + 4 * d->n + 1024);
-        if (want > z->d_out.cap)
-            if (int rc = grow_carrying(ctx, z->d_out, std::max(want, z->d_out.cap * 2), z->produced, retired)) return rc;
+        if (want > z->d_out.cap) call.add(z->d_out, std::max(want, z->d_out.cap * 2), z->produced);
     }
+    if (int rc = call.grow(staged)) return rc;
+    // the host keeps the input from the resume point's byte on, which is all stored_in_flight reads
+    if (int rc = call.stage(live, &pngb200_inflator_push_desc::inflator, [](pngb200_inflator_push_desc* d) {
+            pngb200_inflator* z = d->inflator;
+            const uint64_t decoded = std::min<uint64_t>((z->resume_bit >> 3) - z->tail_at, z->tail.size());
+            z->tail.erase(z->tail.begin(), z->tail.begin() + (ptrdiff_t)decoded);
+            z->tail_at += decoded;
+            z->tail.insert(z->tail.end(), d->data, d->data + d->n);
+            z->pushed += d->n;
+        }))
+        return rc;
     // Rounds: every live handle decodes once; a handle whose output ran out grows it and goes again in the next round.
     constexpr uint64_t kWave = 64u << 10;
     std::vector<pngb200_inflator_push_desc*> round = live;
@@ -2195,9 +2209,7 @@ int inflate_pushes(pngb200_ctx* ctx, pngb200_inflator_push_desc* const* items, s
         // A push with a lot of undecoded input goes through the intra-stream parallel kernel (one CTA: ~25 x the
         // lock-step warp); short ones, and what is left of the wave the input ends in, through the serial decoder.
         // Both resume where the last push stopped: at a block header, or at the last complete symbol of a Huffman block.
-        auto pending = [](const pngb200_inflator* z) {
-            return z->input.size() - std::min<uint64_t>(z->input.size(), z->resume_bit >> 3);
-        };
+        auto pending = [](const pngb200_inflator* z) { return z->pushed - std::min<uint64_t>(z->pushed, z->resume_bit >> 3); };
         std::stable_partition(round.begin(), round.end(),
                               [&](const pngb200_inflator_push_desc* d) { return pending(d->inflator) >= kWave; });
         const size_t m = round.size();
@@ -2208,7 +2220,7 @@ int inflate_pushes(pngb200_ctx* ctx, pngb200_inflator_push_desc* const* items, s
         std::vector<ResumePoint>  at(m);
         for (size_t k = 0; k < m; ++k) {
             pngb200_inflator* z = round[k]->inflator;
-            jobs[k] = whole_stream_job(z->d_in.as<uint8_t>(), z->input.size(), z->d_out.as<uint8_t>(), z->d_out.cap, z->format);
+            jobs[k] = whole_stream_job(z->d_in.as<uint8_t>(), z->pushed, z->d_out.as<uint8_t>(), z->d_out.cap, z->format);
             jobs[k].start_bit = z->resume_bit;
             jobs[k].start_out = z->resume_out;
             jobs[k].phase = (int32_t)z->phase;
@@ -2279,7 +2291,7 @@ int inflate_pushes(pngb200_ctx* ctx, pngb200_inflator_push_desc* const* items, s
             z->resume_out = r.resume_out;
             if (r.status == PNGB200_ERR_OUTPUT_CAPACITY) {
                 z->produced = r.resume_out;
-                if (int rc = grow_carrying(ctx, z->d_out, z->d_out.cap * 2, z->produced, retired)) return rc;
+                call.add(z->d_out, z->d_out.cap * 2, z->produced);
                 again.push_back(round[k]);
                 continue;
             }
@@ -2290,9 +2302,10 @@ int inflate_pushes(pngb200_ctx* ctx, pngb200_inflator_push_desc* const* items, s
             if (r.status == PNGB200_OK) z->terminal = true;
             round[k]->status = r.status;
         }
+        if (int rc = call.grow(0)) return rc;
         round.swap(again);
     }
-    return PNGB200_OK;
+    return call.done();
 }
 
 }  // namespace
@@ -2304,12 +2317,7 @@ int pngb200_inflator_push_batch(pngb200_ctx* ctx, pngb200_inflator_push_desc* pu
     if (int rc = check_pushes(ctx, pushes, count, &pngb200_inflator_push_desc::inflator, "inflator_push_batch")) return rc;
     if (!count) return PNGB200_OK;
     DeviceGuard guard(ctx->device);
-    std::vector<pngb200_inflator_push_desc*> items(count);
-    for (size_t i = 0; i < count; ++i) items[i] = &pushes[i];
-    std::vector<DevBuf> retired;
-    const int rc = inflate_pushes(ctx, items.data(), count, retired);
-    if (rc != PNGB200_OK) cudaStreamSynchronize(ctx->stream);   // before `retired` frees what the stream may still read
-    return rc;
+    return inflate_pushes(ctx, pushes, count);
 }
 
 int pngb200_inflator_push(pngb200_inflator* z, const uint8_t* data, size_t n)
@@ -2446,18 +2454,18 @@ void pngb200_png_context_destroy(pngb200_png_context* c)
 // Filtered bytes the reference's inflator makes available for the input pushed so far, beyond the inflator handle's
 // `produced`: the handle leaves a stored block whose payload has not fully arrived for the next push, while
 // LZ77.Inflator releases its payload byte by byte (Stream.readBlock(upTo:), Stream.swift:384-399).  Sets *src to
-// where those bytes start in the input.
+// where those bytes start in the input.  Reads the block's header from the handle's undecoded tail.
 static uint64_t stored_in_flight(const pngb200_inflator* z, uint64_t* src)
 {
     if (z->terminal || z->status < 0 || z->phase != 1 || z->produced != z->resume_out) return 0;
-    const std::vector<uint8_t>& in = z->input;
-    const uint64_t b = z->resume_bit, bits = 8 * (uint64_t)in.size();
-    if (b + 3 > bits || ((in[(b + 1) >> 3] >> ((b + 1) & 7)) & 1) || ((in[(b + 2) >> 3] >> ((b + 2) & 7)) & 1)) return 0;
+    auto in = [z](uint64_t i) { return z->tail[i - z->tail_at]; };
+    const uint64_t b = z->resume_bit, bits = 8 * z->pushed;
+    if (b + 3 > bits || ((in((b + 1) >> 3) >> ((b + 1) & 7)) & 1) || ((in((b + 2) >> 3) >> ((b + 2) & 7)) & 1)) return 0;
     const uint64_t boundary = (b + 3 + 7) & ~(uint64_t)7;
     if (boundary + 32 > bits) return 0;
-    const uint64_t len = in[boundary >> 3] | ((uint64_t)in[(boundary >> 3) + 1] << 8);
+    const uint64_t len = in(boundary >> 3) | ((uint64_t)in((boundary >> 3) + 1) << 8);
     *src = (boundary >> 3) + 4;
-    return std::min<uint64_t>(len, in.size() - *src);
+    return std::min<uint64_t>(len, z->pushed - *src);
 }
 
 }  // extern "C"
@@ -2472,7 +2480,7 @@ struct ContextRange { int z; uint64_t r0, r1; };
 // every context are reconstructed by one unfilter_pass_kernel launch and assigned by at most seven
 // context_assign_batch_kernel launches, the k-th over the k-th pass range of every context.  Statuses as in
 // inflate_pushes.
-int context_pushes(pngb200_ctx* ctx, pngb200_png_push_desc* pushes, size_t count, std::vector<DevBuf>& retired)
+int context_pushes(pngb200_ctx* ctx, pngb200_png_push_desc* pushes, size_t count)
 {
     std::vector<pngb200_png_push_desc*>      live;
     std::vector<pngb200_inflator_push_desc>  zp;
@@ -2489,9 +2497,8 @@ int context_pushes(pngb200_ctx* ctx, pngb200_png_push_desc* pushes, size_t count
         }
     }
     if (live.empty()) return PNGB200_OK;
-    std::vector<pngb200_inflator_push_desc*> zi(zp.size());
-    for (size_t k = 0; k < zp.size(); ++k) zi[k] = &zp[k];
-    const int irc = inflate_pushes(ctx, zi.data(), zi.size(), retired);
+    PushCall call(ctx);   // grows nothing: synchronises on the way out of a failed call
+    const int irc = inflate_pushes(ctx, zp.data(), zp.size());
     std::vector<pngb200_png_push_desc*>   rowed;    // the pushes whose inflate succeeded
     std::vector<uint64_t>                 avail;    // filtered bytes the reference has released after each of them
     std::vector<std::vector<ContextRange>> ranges;
@@ -2637,7 +2644,7 @@ int context_pushes(pngb200_ctx* ctx, pngb200_png_push_desc* pushes, size_t count
             rowed[i]->status = PNGB200_ERR_PNG_EXTRANEOUS_IMAGE_DATA;
         }
     }
-    return PNGB200_OK;
+    return call.done();
 }
 
 }  // namespace
@@ -2650,10 +2657,7 @@ int pngb200_png_context_push_batch(pngb200_ctx* ctx, pngb200_png_push_desc* push
     if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_context_push: a decode batch is pending");
     if (!count) return PNGB200_OK;
     DeviceGuard guard(ctx->device);
-    std::vector<DevBuf> retired;
-    const int rc = context_pushes(ctx, pushes, count, retired);
-    if (rc != PNGB200_OK) cudaStreamSynchronize(ctx->stream);   // before `retired` frees what the stream may still read
-    return rc;
+    return context_pushes(ctx, pushes, count);
 }
 
 int pngb200_png_context_push(pngb200_png_context* c, const uint8_t* data, size_t n, int overdraw)
