@@ -573,6 +573,80 @@ int    pngb200_deflator_pop(pngb200_deflator* z, const uint8_t** block, size_t* 
 /* pull() : a complete block if there is one, else the flushed incomplete block (non-empty); 0 = nil */
 int    pngb200_deflator_pull(pngb200_deflator* z, const uint8_t** block, size_t* n);
 
+/* ---- online encoding: PNG.Image.compress(stream:level:hint:) row by row (Sources/PNG/PNG.Image.swift:576-668,
+ * PNG.Encoder.pull, Sources/PNG/Encoding/PNG.Encoder.swift:33-129) --------------------------------------------------
+ * A caller pushes the rows of PNG.Image.storage as they are produced, top to bottom; the handle collects and filters
+ * the scanlines they complete on the device (filter_resume_kernel, one warp a scanline, straight onto the end of an
+ * online deflator's input), deflates them (deflate_resume_kernel), CRCs the IDAT payload on the device
+ * (crc_regions_kernel) and frames the chunks.  pop() then hands out the file in pieces:
+ *   1. the head: signature, [CgBI], IHDR, [PLTE], [tRNS], as pngb200_png_encode_files writes it -- a piece of its own,
+ *      so that a caller can splice ancillary chunks in behind it;
+ *   2. each IDAT chunk, framed (length, type, payload of idat_chunk bytes, the last one shorter, CRC-32);
+ *   3. IEND.
+ * For every push schedule the pieces joined are pngb200_png_encode_batch's file for the same image, level and
+ * idat_chunk.  After each push the pieces available are exactly the chunks the reference has written by the time
+ * PNG.Encoder.pull asks collect for the first scanline the rows pushed so far do not complete: a non-interlaced
+ * scanline y needs storage row y; Adam7 pass z's scanline y needs row by + y * sy, in stream order (pass 0 streams
+ * while rows arrive, the others follow as the rows they need arrive).  The reference pushes one scanline at a time
+ * into its deflator, and each of those pushes compresses when more than 4096 bytes are pending, so the deflate kernel
+ * applies that rule at every scanline end inside a push.  The push that brings the last row also does
+ * push([], last: true): the rest of the payload and IEND become available.
+ * Device memory: the online deflator's (its dictionary, the input from min(block start, window start) on and, at
+ * levels 8-13, the unfinished block's graph; see pngb200_deflator_create_online), plus one storage row for a
+ * non-interlaced image -- independent of the image's height -- or the whole storage for an Adam7 image, since passes
+ * 1 to 6 reread rows pass 0 used.
+ * Size limit: one push completes at most 1 GiB of filtered scanlines (the online deflator's limit on one push).  So
+ * pngb200_png_encoder_create refuses a non-interlaced image whose filtered scanline (pitch + 1 bytes) is over 1 GiB,
+ * and an Adam7 image whose whole filtered stream (pngb200_filtered_size) is over 1 GiB, since its last row completes
+ * passes 1 to 6 at once.  pngb200_png_encode_batch encodes such images. */
+typedef struct pngb200_png_encoder pngb200_png_encoder;
+typedef struct pngb200_png_encoder_desc {
+    uint32_t             width, height;
+    pngb200_pixel_format format;       /* bgr = 1 writes the ios standard (CgBI chunk, raw deflate) */
+    uint8_t              interlaced;
+    int32_t              level;        /* 0...13 */
+    uint32_t             idat_chunk;   /* bytes per IDAT chunk; 0 = 65544, as pngb200_png_encode_desc */
+} pngb200_png_encoder_desc;
+/* Validation as pngb200_png_encode_files, plus the size limit above; NULL with the reason in the last error on failure
+ * (a bad descriptor or an image over the limit: PNGB200_ERR_BAD_ARGUMENT; no device memory: PNGB200_ERR_CUDA).  The palette is read during the call only. */
+pngb200_png_encoder* pngb200_png_encoder_create(pngb200_ctx* ctx, const pngb200_png_encoder_desc* desc);
+void                 pngb200_png_encoder_destroy(pngb200_png_encoder* e);
+/* `rows`: the next n bytes of storage, a whole number of rows (zero included), in `memspace` (PNGB200_MEM_DEVICE: the
+ * context's GPU, read in place).  pngb200_png_encoder_push_batch with one item. */
+int  pngb200_png_encoder_push(pngb200_png_encoder* e, const void* rows, size_t n, int memspace);
+/* Many pushes in one call, one per encoder.  Each item behaves exactly as the same push made alone: its status,
+ * pieces and progress are the ones that push would leave.  Items may mix formats, levels, interlacing, idat_chunk and
+ * memspaces.  Returns PNGB200_ERR_BAD_ARGUMENT, touching no item, for a null ctx or array, a null handle, a handle of
+ * another ctx, the same handle twice, rows NULL with n > 0, a memspace other than HOST or DEVICE, or a pending decode
+ * batch; PNGB200_ERR_CUDA, with every handle unchanged, when a buffer cannot be allocated.  Otherwise each item's
+ * status is PNGB200_OK or: PNGB200_ERR_BAD_ARGUMENT for n that is not a whole number of rows, rows past the height,
+ * a push after the image is complete, or a push of many non-interlaced rows that completes more than 1 GiB of filtered
+ * scanlines (the handle is unchanged: the same rows pushed in smaller bands go through); the handle's sticky error if an earlier push failed on
+ * the device; a device error, which then sticks.
+ * Cost per call: kernel launches and synchronises are fixed whatever `count` -- at most one filter_resume_kernel, one
+ * deflate_resume_kernel and one crc_regions_kernel launch, and at most two stream synchronises.  Copies: one upload of
+ * all host rows and one of the launch tables; when new payload bytes were written, one upload of the CRC-32 regions,
+ * one clear and one readback of their CRCs; and per item with rows, one device-to-device copy (Adam7: its rows into
+ * the handle's storage; otherwise its last row into the carried row, except on the push that completes the image).
+ * A device error once the call's buffers are allocated makes every item's handle error sticky. */
+typedef struct pngb200_png_encoder_push_desc {
+    pngb200_png_encoder* encoder;
+    const void*          rows;
+    size_t               n;
+    int32_t              memspace;    /* pngb200_memspace of `rows` */
+    int32_t              status;      /* out */
+} pngb200_png_encoder_push_desc;
+int  pngb200_png_encoder_push_batch(pngb200_ctx* ctx, pngb200_png_encoder_push_desc* pushes, size_t count);
+/* The next piece of the file: returns 1 and sets *bytes / *n (valid until the next call on this handle), or 0 when
+ * there is none now (nil). */
+int  pngb200_png_encoder_pop(pngb200_png_encoder* e, const uint8_t** bytes, size_t* n);
+/* out[0] storage rows received; out[1] scanlines filtered and given to the deflator, in stream order; out[2] filtered
+ * bytes the deflator has dequeued; out[3] IDAT chunks handed out by pop(); out[4] 1 once IEND is available; out[5]
+ * device bytes the handle holds now. */
+int  pngb200_png_encoder_progress(const pngb200_png_encoder* e, uint64_t out[6]);
+/* the sticky device error (PNGB200_OK if none); a and b are 0 (kept for the shape of the other handles' calls) */
+void pngb200_png_encoder_error(const pngb200_png_encoder* e, int* status, uint32_t* a, uint32_t* b);
+
 #ifdef __cplusplus
 }
 #endif

@@ -192,6 +192,16 @@ class PngPushDesc(C.Structure):
                 ("status", C.c_int32)]
 
 
+class PngEncoderDesc(C.Structure):
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("format", PixelFormat), ("interlaced", C.c_uint8),
+                ("level", C.c_int32), ("idat_chunk", C.c_uint32)]
+
+
+class PngEncoderPushDesc(C.Structure):
+    _fields_ = [("encoder", C.c_void_p), ("rows", C.c_void_p), ("n", C.c_size_t), ("memspace", C.c_int32),
+                ("status", C.c_int32)]
+
+
 class PNGB200Error(RuntimeError):
     def __init__(self, status: int, message: str = ""):
         super().__init__(f"pngb200 status {status}: {message}")
@@ -343,6 +353,22 @@ def lib():
         L.pngb200_inflator_push_batch.restype = C.c_int
         L.pngb200_png_context_push_batch.argtypes = [C.c_void_p, C.POINTER(PngPushDesc), C.c_size_t]
         L.pngb200_png_context_push_batch.restype = C.c_int
+    if hasattr(L, "pngb200_png_encoder_create"):
+        L.pngb200_png_encoder_create.argtypes = [C.c_void_p, C.POINTER(PngEncoderDesc)]
+        L.pngb200_png_encoder_create.restype = C.c_void_p
+        L.pngb200_png_encoder_destroy.argtypes = [C.c_void_p]
+        L.pngb200_png_encoder_destroy.restype = None
+        L.pngb200_png_encoder_push.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]
+        L.pngb200_png_encoder_push.restype = C.c_int
+        L.pngb200_png_encoder_push_batch.argtypes = [C.c_void_p, C.POINTER(PngEncoderPushDesc), C.c_size_t]
+        L.pngb200_png_encoder_push_batch.restype = C.c_int
+        L.pngb200_png_encoder_pop.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t)]
+        L.pngb200_png_encoder_pop.restype = C.c_int
+        L.pngb200_png_encoder_progress.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.pngb200_png_encoder_progress.restype = C.c_int
+        L.pngb200_png_encoder_error.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_uint32),
+                                                C.POINTER(C.c_uint32)]
+        L.pngb200_png_encoder_error.restype = None
     _lib = L
     return L
 
@@ -1040,3 +1066,77 @@ def png_context_push_batch(ctx: Context, items) -> list:
     contexts of `ctx`.  Returns each push's status, as PngContext.push would raise it (payloads through the context's
     error()); raises PNGB200Error only when the call itself fails."""
     return _push_batch(ctx, PngPushDesc, ctx._lib.pngb200_png_context_push_batch, items)
+
+
+class PngEncoder:
+    """PNG.Image.compress(stream:level:) online on the GPU: push the rows of PNG.Image.storage as they are produced, top
+    to bottom, and pop() the file in pieces (the head, each IDAT chunk, IEND) as soon as the reference would have
+    written them.  The format fields are those of png_encode_batch's image dicts."""
+
+    def __init__(self, ctx: Context, width: int, height: int, color: int, depth: int, bgr: bool = False, key=None,
+                 palette=None, interlaced: bool = False, level: int = 9, idat_chunk: int = 0):
+        self.ctx = ctx
+        d, keep = PngEncoderDesc(width=width, height=height, interlaced=int(bool(interlaced)), level=level,
+                                 idat_chunk=idat_chunk), []
+        _fill_format(d.format, keep, color, depth, bgr, key, palette)
+        self.handle = ctx._lib.pngb200_png_encoder_create(ctx.handle, C.byref(d))
+        if not self.handle:
+            raise PNGB200Error(ERR_BAD_ARGUMENT, ctx._lib.pngb200_last_error(ctx.handle).decode())
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.ctx._lib.pngb200_png_encoder_destroy(self.handle)
+            self.handle = None
+
+    __del__ = close
+
+    def push(self, rows, memspace: int = MEM_HOST) -> None:
+        """the next whole rows of storage: bytes (MEM_HOST), or (address, length) on the context's GPU (MEM_DEVICE)"""
+        (st,) = png_encoder_push_batch(self.ctx, [(self, rows, memspace)])
+        if st < 0:
+            raise PNGB200Error(st, self.ctx._lib.pngb200_last_error(self.ctx.handle).decode())
+
+    def pop(self):
+        """the next piece of the file, or None when there is none now"""
+        p, n = C.POINTER(C.c_uint8)(), C.c_size_t()
+        got = self.ctx._lib.pngb200_png_encoder_pop(self.handle, C.byref(p), C.byref(n))
+        if got < 0:
+            raise PNGB200Error(got, "png_encoder_pop")
+        return C.string_at(p, n.value) if got else None
+
+    def pop_all(self) -> list:
+        out = []
+        while (piece := self.pop()) is not None:
+            out.append(piece)
+        return out
+
+    def progress(self) -> tuple:
+        """(rows received, scanlines filtered, filtered bytes dequeued, IDAT chunks popped, IEND available, device
+        bytes held)"""
+        out = (C.c_uint64 * 6)()
+        self.ctx.check(self.ctx._lib.pngb200_png_encoder_progress(self.handle, out))
+        return tuple(out)
+
+    def error(self) -> int:
+        s, a, b = C.c_int(), C.c_uint32(), C.c_uint32()
+        self.ctx._lib.pngb200_png_encoder_error(self.handle, C.byref(s), C.byref(a), C.byref(b))
+        return s.value
+
+
+def png_encoder_push_batch(ctx: Context, items) -> list:
+    """pushes of many PngEncoders in one call: `items` is [(encoder, rows[, memspace])], distinct encoders of `ctx`,
+    rows as PngEncoder.push takes them.  Returns each push's status; raises PNGB200Error only when the call itself
+    fails."""
+    descs = (PngEncoderPushDesc * max(len(items), 1))()
+    keep = []
+    for d, item in zip(descs, items):
+        mem = item[2] if len(item) > 2 else MEM_HOST
+        d.encoder, d.memspace = item[0].handle, mem
+        if mem == MEM_DEVICE:
+            d.rows, d.n = int(item[1][0]) or None, int(item[1][1])
+        else:
+            data = bytes(item[1])
+            keep.append(data)
+            d.rows, d.n = C.cast(C.c_char_p(data), C.c_void_p), len(data)
+    ctx.check(ctx._lib.pngb200_png_encoder_push_batch(ctx.handle, descs, len(items)))
+    return [descs[i].status for i in range(len(items))]

@@ -962,6 +962,15 @@ struct DfResumeJob {
     struct DfResumeResult* result;   // pinned host memory
     int32_t   format, level, exponent, last;
 };
+// The scanline ends of a push (pngb200_png_encoder_push_batch), positions relative to the carry's base in increasing
+// order, the last one the job's n.  PNG.Encoder.pull pushes one scanline at a time into its deflator, and each of those
+// pushes compresses when more than 4096 bytes are pending (DeflatorBuffers.swift:74): the kernel walks the ends and does
+// the same at each, so it releases blocks no earlier than the reference.  It is an array beside the jobs, so that a
+// DfResumeJob keeps its layout.
+struct DfEnds {
+    const uint64_t* at;
+    uint64_t        count;
+};
 struct DfResumeResult {
     int32_t  status;
     uint32_t blocks;           // blocks written by this launch
@@ -982,7 +991,8 @@ inline void df_carry_init(DfCarry& c)
 }
 constexpr size_t DF_DICT_WORDS = (1u << DF_HASH_BITS) + 2 * 32768;
 
-__global__ void __launch_bounds__(32) deflate_resume_kernel(const DfResumeJob* jobs, int count)
+// `ends`: null, or one DfEnds per job; a job whose ends are null, or a launch without them, has one end at n.
+__global__ void __launch_bounds__(32) deflate_resume_kernel(const DfResumeJob* jobs, int count, const DfEnds* ends = nullptr)
 {
     PNGB200_DYN_SMEM(df_smem);
     DfShared& S = *reinterpret_cast<DfShared*>(df_smem);
@@ -1039,15 +1049,25 @@ __global__ void __launch_bounds__(32) deflate_resume_kernel(const DfResumeJob* j
                 df_write_stored(out, z.x, z.n);   // never compacted: a stream this short has base 0
                 ++blocks;
             } else {
-                const int64_t lookahead = job.last ? 0 : z.mode == 1 ? 259 : 258;
-                for (;;) {
-                    const bool full = df_compress(z, S, lookahead);
-                    if (!full && !job.last) break;
-                    const int rc = df_write_block(z, S, out, !full);
-                    ++blocks;
-                    if (rc) { status = rc; break; }
-                    if (!full) break;
+                const DfEnds  e = ends ? ends[t] : DfEnds{nullptr, 0};
+                const uint64_t nends = e.at ? e.count : 1;
+                for (uint64_t k = 0; k < nends && status == PNGB200_OK; ++k) {
+                    const bool last = job.last && k + 1 == nends;
+                    if (e.at) {
+                        z.n = (int64_t)e.at[k];
+                        if (!last && df_input_count(z) <= 4096) continue;   // DeflatorBuffers.swift:74
+                    }
+                    const int64_t lookahead = last ? 0 : z.mode == 1 ? 259 : 258;
+                    for (;;) {
+                        const bool full = df_compress(z, S, lookahead);
+                        if (!full && !last) break;
+                        const int rc = df_write_block(z, S, out, !full);
+                        ++blocks;
+                        if (rc) { status = rc; break; }
+                        if (!full) break;
+                    }
                 }
+                z.n = (int64_t)job.n;
             }
             if (job.last && job.format == PNGB200_FORMAT_ZLIB) {
                 const uint32_t ck = s2 << 16 | s1;

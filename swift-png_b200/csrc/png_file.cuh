@@ -44,6 +44,65 @@ void take_walk(const WalkHead& h, const uint8_t* palette, pngb200_png_desc& d, F
     w.first_idat = (size_t)h.first_idat, w.idat_end = (size_t)h.idat_end;
 }
 
+// one chunk onto `h`: length, type, body and CRC-32 (these few bytes are CRC'd where they are built)
+void put_chunk(std::vector<uint8_t>& h, uint32_t type, const uint8_t* body, size_t n)
+{
+    const size_t at = h.size();
+    h.resize(at + 12 + n);
+    store_be32(h.data() + at, (uint32_t)n), store_be32(h.data() + at + 4, type);
+    if (n) memcpy(h.data() + at + 8, body, n);
+    uint32_t c = 0xffffffffu;
+    for (size_t k = at + 4; k < at + 8 + n; ++k) {
+        c ^= h[k];
+        for (int b = 0; b < 8; ++b) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
+    }
+    store_be32(h.data() + at + 8 + n, ~c);
+}
+
+// Everything in front of the first IDAT, built on the host (a few hundred bytes): signature, [CgBI], IHDR, [PLTE],
+// [tRNS]  (PNG.Image.swift:580-629, PNG.Image.encode :416-423, Layout.palette / Layout.transparency,
+// Formats/PNG.Layout.swift:43-135)
+void png_head(const pngb200_pixel_format& f, uint32_t width, uint32_t height, int interlaced, std::vector<uint8_t>& h)
+{
+    h.assign(PNG_SIGNATURE, PNG_SIGNATURE + 8);
+    if (f.bgr) {
+        const uint8_t cgbi[4] = {48, 0, 32, (uint8_t)(f.color == 2 ? 6 : 2)};
+        put_chunk(h, CK_CgBI, cgbi, 4);
+    }
+    uint8_t ihdr[13];
+    store_be32(ihdr, width), store_be32(ihdr + 4, height);
+    ihdr[8] = f.depth, ihdr[9] = f.color, ihdr[10] = 0, ihdr[11] = 0, ihdr[12] = interlaced ? 1 : 0;
+    put_chunk(h, CK_IHDR, ihdr, 13);
+    if (f.color == 3) {
+        uint8_t rgb[768], alpha[256];
+        int last = -1;
+        for (int k = 0; k < f.palette_count; ++k) {
+            memcpy(rgb + 3 * k, f.palette + 4 * k, 3);
+            alpha[k] = f.palette[4 * k + 3];
+            if (alpha[k] != 255) last = k;
+        }
+        put_chunk(h, CK_PLTE, rgb, 3 * (size_t)f.palette_count);
+        if (last >= 0) put_chunk(h, CK_tRNS, alpha, (size_t)last + 1);
+    } else if (f.has_key && (f.color == 0 || f.color == 2)) {
+        uint8_t k[6];
+        if (f.color == 0) {
+            k[0] = (uint8_t)(f.key[0] >> 8), k[1] = (uint8_t)f.key[0];
+            put_chunk(h, CK_tRNS, k, 2);
+        } else {
+            const uint16_t r = f.bgr ? f.key[2] : f.key[0], g = f.key[1], b = f.bgr ? f.key[0] : f.key[2];
+            k[0] = (uint8_t)(r >> 8), k[1] = (uint8_t)r, k[2] = (uint8_t)(g >> 8), k[3] = (uint8_t)g, k[4] = (uint8_t)(b >> 8), k[5] = (uint8_t)b;
+            put_chunk(h, CK_tRNS, k, 6);
+        }
+    }
+}
+
+// the format checks of pngb200_png_encode_files: a pixel format the PNG layout allows, a palette that fits its depth
+bool encode_format_ok(const pngb200_pixel_format& f, uint32_t width, uint32_t height)
+{
+    return pixel_rule(f.color, f.depth, f.bgr).valid && width && height &&
+           !(f.color == 3 && (!f.palette || !f.palette_count || f.palette_count > (1u << f.depth)));
+}
+
 struct RecordVector {
     std::vector<ChunkRec>* v;
     void put(uint64_t, const ChunkRec& r) const { v->push_back(r); }
@@ -528,11 +587,9 @@ int pngb200_png_encode_files(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_
     Slots pixels{16}, payloads{16};
     for (size_t i = 0; i < count; ++i) {
         const pngb200_pixel_format& f = d[i].format;
-        const PixelRule rule = pixel_rule(f.color, f.depth, f.bgr);
-        if (!rule.valid || !d[i].width || !d[i].height || !d[i].pixels || !d[i].file ||
-            (f.color == 3 && (!f.palette || !f.palette_count || f.palette_count > (1u << f.depth))))
+        if (!encode_format_ok(f, d[i].width, d[i].height) || !d[i].pixels || !d[i].file)
             return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: bad descriptor", i);
-        const int    volume = f.depth * rule.channels;
+        const int    volume = f.depth * pixel_rule(f.color, f.depth, f.bgr).channels;
         const size_t storage = pngb200_storage_size(d[i].width, d[i].height, volume);
         if (d[i].pixels_len < storage) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "image %zu: pixels_len", i);
         if (d[i].file_cap < pngb200_png_encode_bound(d[i].width, d[i].height, &f, d[i].interlaced, d[i].idat_chunk))
@@ -561,52 +618,8 @@ int pngb200_png_encode_files(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_
         e.volume = (uint8_t)volume, e.depth = f.depth, e.interlaced = d[i].interlaced;
         e.format = f.bgr ? PNGB200_FORMAT_IOS : PNGB200_FORMAT_ZLIB;
         e.level = d[i].level;
-        // everything in front of the first IDAT, built on the host (a few hundred bytes):
-        // signature, [CgBI], IHDR, [PLTE], [tRNS]  (PNG.Image.swift:580-629, PNG.Image.encode :416-423,
-        // Layout.palette / Layout.transparency, Formats/PNG.Layout.swift:43-135)
-        std::vector<uint8_t>& h = heads[i];
-        auto put = [&](uint32_t type, const uint8_t* body, size_t n) {
-            const size_t at = h.size();
-            h.resize(at + 12 + n);
-            store_be32(h.data() + at, (uint32_t)n), store_be32(h.data() + at + 4, type);
-            if (n) memcpy(h.data() + at + 8, body, n);
-            uint32_t c = 0xffffffffu;  // these few bytes are CRC'd where they are built
-            for (size_t k = at + 4; k < at + 8 + n; ++k) {
-                c ^= h[k];
-                for (int b = 0; b < 8; ++b) c = (c & 1) ? 0xEDB88320u ^ (c >> 1) : c >> 1;
-            }
-            store_be32(h.data() + at + 8 + n, ~c);
-        };
-        h.assign(PNG_SIGNATURE, PNG_SIGNATURE + 8);
-        if (f.bgr) {
-            const uint8_t cgbi[4] = {48, 0, 32, (uint8_t)(f.color == 2 ? 6 : 2)};
-            put(CK_CgBI, cgbi, 4);
-        }
-        uint8_t ihdr[13];
-        store_be32(ihdr, d[i].width), store_be32(ihdr + 4, d[i].height);
-        ihdr[8] = f.depth, ihdr[9] = f.color, ihdr[10] = 0, ihdr[11] = 0, ihdr[12] = d[i].interlaced ? 1 : 0;
-        put(CK_IHDR, ihdr, 13);
-        if (f.color == 3) {
-            uint8_t rgb[768], alpha[256];
-            int last = -1;
-            for (int k = 0; k < f.palette_count; ++k) {
-                memcpy(rgb + 3 * k, f.palette + 4 * k, 3);
-                alpha[k] = f.palette[4 * k + 3];
-                if (alpha[k] != 255) last = k;
-            }
-            put(CK_PLTE, rgb, 3 * (size_t)f.palette_count);
-            if (last >= 0) put(CK_tRNS, alpha, (size_t)last + 1);
-        } else if (f.has_key && (f.color == 0 || f.color == 2)) {
-            uint8_t k[6];
-            if (f.color == 0) {
-                k[0] = (uint8_t)(f.key[0] >> 8), k[1] = (uint8_t)f.key[0];
-                put(CK_tRNS, k, 2);
-            } else {
-                const uint16_t r = f.bgr ? f.key[2] : f.key[0], g = f.key[1], b = f.bgr ? f.key[0] : f.key[2];
-                k[0] = (uint8_t)(r >> 8), k[1] = (uint8_t)r, k[2] = (uint8_t)(g >> 8), k[3] = (uint8_t)g, k[4] = (uint8_t)(b >> 8), k[5] = (uint8_t)b;
-                put(CK_tRNS, k, 6);
-            }
-        }
+        png_head(f, d[i].width, d[i].height, d[i].interlaced, heads[i]);
+        const std::vector<uint8_t>& h = heads[i];
         head_len[i] = h.size();
     }
     int rc = pngb200_encode_batch(ctx, enc.data(), count, PNGB200_MEM_DEVICE);
@@ -677,6 +690,420 @@ int pngb200_png_encode_files(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_
 int pngb200_png_encode_batch(pngb200_ctx* ctx, pngb200_png_encode_desc* d, size_t count, int memspace)
 {
     return pngb200_png_encode_files(ctx, d, count, memspace, PNGB200_MEM_HOST);
+}
+
+}  // extern "C"
+
+// ---------------- online encoding: PNG.Encoder.pull as the rows arrive ----------------
+// The handle owns an online deflator; each push filters the scanlines it completes onto the end of the deflator's
+// input, deflates them (scanline ends in DfEnds), CRCs the new payload bytes on the device and frames the chunks that
+// the deflator's pop() / pull() now hand out.
+struct pngb200_png_encoder {
+    pngb200_ctx*      ctx = nullptr;
+    pngb200_deflator* z = nullptr;
+    uint32_t width = 0, height = 0;
+    uint8_t  volume = 0, depth = 0, interlaced = 0, bpp = 0;
+    uint64_t row_bytes = 0;            // storage bytes a row
+    uint64_t rows = 0;                 // storage rows received
+    uint64_t lines = 0;                // stream scanlines filtered
+    DevBuf   d_rows;                   // non-interlaced: the last row received; Adam7: the whole storage
+    DevBuf   d_header;                 // the deflate stream's header (zlib: 2 bytes), CRC'd with the first chunk
+    uint64_t header = 0;
+    int      status = PNGB200_OK;      // sticky: a failed launch leaves the device state unknown
+    // IDAT CRC-32s: stream bytes CRC'd so far, the open chunk's CRC (its type included), the finished chunks' CRCs
+    uint64_t crc_at = 0;
+    uint32_t crc_open = 0;
+    std::deque<uint32_t> crcs;
+    std::deque<std::vector<uint8_t>> pieces;   // framed, not popped yet
+    std::vector<uint8_t> popped;               // the piece pop() handed out last
+    uint64_t idat_out = 0;
+    bool     iend = false;
+    size_t device_bytes() const { return z->device_bytes() + d_rows.cap + d_header.cap; }
+    // the first stream scanline that needs a storage row at or past `r` (Adam7: pass z's scanline y reads row
+    // by + y * sy), and the stream offset of scanline `line`
+    uint64_t lines_complete(uint64_t r) const
+    {
+        uint64_t n = 0;
+        for (int p = 0; p < 7; ++p) {
+            const Pass ps = stream_pass(p, width, height, volume, interlaced);
+            const uint64_t got = r > ps.by ? std::min<uint64_t>(ps.height, ((r - 1 - ps.by) >> ps.ey) + 1) : 0;
+            n += got;
+            if (got < ps.height) break;
+        }
+        return n;
+    }
+    uint64_t line_offset(uint64_t line) const
+    {
+        uint64_t off = 0;
+        for (int p = 0; p < 7; ++p) {
+            const Pass ps = stream_pass(p, width, height, volume, interlaced);
+            const uint64_t k = std::min<uint64_t>(line, ps.height);
+            off += k * (ps.pitch + 1);
+            line -= k;
+        }
+        return off;
+    }
+    uint64_t line_end(uint64_t line) const { return line_offset(line + 1); }
+};
+
+namespace {
+
+// crc(A || B) from crc(A), crc(B) and |B| (crc32.cuh: multiply crc(A) by x^(8|B|))
+uint32_t crc_combine(uint32_t a, uint32_t b, uint64_t nb)
+{
+    static const std::vector<uint32_t> t = [] {
+        std::vector<uint32_t> v(CRC_TABLE_WORDS);
+        crc_build_tables(v.data());
+        return v;
+    }();
+    for (int k = 0; nb && a; nb >>= 1, ++k) {
+        if (!(nb & 1)) continue;
+        uint32_t s = 0;
+        for (int i = 0; i < 32; ++i)
+            if (a >> i & 1) s ^= t[256 + 32 * k + i];
+        a = s;
+    }
+    return a ^ b;
+}
+
+// one IDAT chunk from the deflator's bytes and the CRC the device computed for it
+std::vector<uint8_t> frame_idat(const uint8_t* body, size_t n, uint32_t crc)
+{
+    std::vector<uint8_t> c(12 + n);
+    store_be32(c.data(), (uint32_t)n), store_be32(c.data() + 4, CK_IDAT);
+    memcpy(c.data() + 8, body, n);
+    store_be32(c.data() + 8 + n, crc);
+    return c;
+}
+
+// The pushes of one pngb200_png_encoder_push_batch call, on distinct encoders of `ctx`
+int encoder_pushes(pngb200_ctx* ctx, pngb200_png_encoder_push_desc* pushes, size_t count)
+{
+    struct Item {
+        pngb200_png_encoder_push_desc* d;
+        pngb200_png_encoder* e;
+        uint64_t rows, lines;          // after the push
+        uint64_t filtered;             // bytes of the scanlines it completes
+        bool     last;
+        DfNeed   need;
+        size_t   staged = 0;           // offset of its host rows in the staging
+        size_t   ends = 0, job = (size_t)-1;
+        uint64_t written = 0;          // the deflator's bytes before the launch
+    };
+    std::vector<Item> live;
+    size_t staged = 0, nlines = 0, nends = 0, run = 0, host_out = 0, nfilter = 0;
+    for (size_t i = 0; i < count; ++i) {
+        pngb200_png_encoder_push_desc* d = &pushes[i];
+        pngb200_png_encoder* e = d->encoder;
+        const uint64_t add = d->n / e->row_bytes;
+        if (e->status < 0) {
+            d->status = e->status;
+            continue;
+        }
+        if (e->rows == e->height)
+            d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_encoder: push after the image is complete");
+        else if (d->n % e->row_bytes || add > e->height - e->rows)
+            d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_encoder: %zu bytes are not whole rows inside the image", d->n);
+        if (e->rows == e->height || d->n % e->row_bytes || add > e->height - e->rows) continue;
+        Item it;
+        it.d = d, it.e = e;
+        it.rows = e->rows + add;
+        it.lines = e->lines_complete(it.rows);
+        it.filtered = e->line_offset(it.lines) - e->line_offset(e->lines);
+        it.last = it.rows == e->height;
+        if (it.filtered > kMaxDeflatorPush) {
+            d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_encoder: a push completes at most 1 GiB of scanlines");
+            continue;
+        }
+        d->status = PNGB200_ERR_CUDA;   // until its push is answered
+        it.need = df_need(e->z, it.filtered, it.last);
+        if (d->memspace == PNGB200_MEM_HOST) it.staged = staged, staged += d->n;
+        if (it.lines > e->lines) ++nfilter, nlines += it.lines - e->lines;
+        if (it.need.run) {
+            it.ends = nends, nends += it.lines - e->lines;
+            host_out += align_up(it.need.out, 256), ++run;
+        }
+        live.push_back(it);
+    }
+    if (nlines >= (1ull << 31)) {
+        for (Item& it : live) it.d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_encoder_push_batch: too many scanlines");
+        return PNGB200_OK;
+    }
+    // the tables of the call, laid out now so that every allocation comes before any device work
+    std::vector<FilterResumeJob> fjobs(nfilter);
+    std::vector<uint32_t>        line_base(nfilter + 1, 0);
+    std::vector<DfResumeJob>     djobs(run);
+    std::vector<DfEnds>          dends(run);
+    std::vector<uint64_t>        ends(nends);
+    Tables t(ctx->h_st, ctx->d_st);
+    const size_t off_f = t.host(fjobs.data(), sizeof(FilterResumeJob) * fjobs.size());
+    const size_t off_lb = t.host(line_base.data(), sizeof(uint32_t) * line_base.size());
+    const size_t off_dj = t.host(djobs.data(), sizeof(DfResumeJob) * djobs.size());
+    const size_t off_de = t.host(dends.data(), sizeof(DfEnds) * dends.size());
+    const size_t off_e = t.host(ends.data(), sizeof(uint64_t) * ends.size());
+    PushCall call(ctx);
+    const size_t res_off = align_up(host_out, 256);
+    CU(ctx->h_dfout.reserve(res_off + sizeof(DfResumeResult) * std::max<size_t>(run, 1)));
+    CU(ctx->h_st.reserve(t.host_end));
+    CU(ctx->d_st.reserve(t.end));
+    for (Item& it : live) df_grow(call, it.e->z, it.need);
+    if (int rc = call.grow(staged)) return rc;
+    // Everything up to the deflate launch.  A failure here leaves every handle of the call with a sticky error: a
+    // deflator may have counted in input that was never written, so its input and the encoder's row counts no longer
+    // agree.
+    auto enqueue = [&]() -> int {
+        // the host rows of every encoder with one upload; Adam7 rows into the encoder's storage
+        if (int rc = call.pack(live.size(), [&](size_t k) {
+                const pngb200_png_encoder_push_desc* d = live[k].d;
+                return std::pair<const void*, size_t>(d->memspace == PNGB200_MEM_HOST ? d->rows : nullptr,
+                                                      d->memspace == PNGB200_MEM_HOST ? d->n : 0);
+            }))
+            return rc;
+        size_t f = 0, out_at = 0, j = 0;
+        for (Item& it : live) {
+            pngb200_png_encoder* e = it.e;
+            pngb200_deflator* z = e->z;
+            const uint8_t* rows = it.d->memspace == PNGB200_MEM_HOST ? ctx->d_stin.as<uint8_t>() + it.staged : (const uint8_t*)it.d->rows;
+            if (e->interlaced && it.d->n)
+                CU(cudaMemcpyAsync(e->d_rows.as<uint8_t>() + e->rows * e->row_bytes, rows, it.d->n, cudaMemcpyDeviceToDevice, ctx->stream));
+            const uint64_t held = z->held(), off0 = e->line_offset(e->lines);
+            if (it.lines > e->lines) {
+                FilterResumeJob& fj = fjobs[f];
+                fj.rows = e->interlaced ? e->d_rows.as<uint8_t>() : rows;
+                fj.carried = e->d_rows.as<uint8_t>();
+                fj.out = z->d_in.as<uint8_t>() + held;
+                fj.out_off0 = off0;
+                fj.width = e->width, fj.height = e->height;
+                fj.first = (uint32_t)e->lines, fj.row0 = (uint32_t)e->rows;
+                fj.volume = e->volume, fj.depth = e->depth, fj.interlaced = e->interlaced, fj.bpp = e->bpp;
+                line_base[f + 1] = line_base[f] + (uint32_t)(it.lines - e->lines);
+                ++f;
+            }
+            z->total += it.filtered;
+            df_drop_popped(z);
+            it.written = z->written;
+            if (!it.need.run) continue;
+            for (uint64_t k = e->lines; k < it.lines; ++k) ends[it.ends + (k - e->lines)] = held + (e->line_end(k) - off0);
+            dends[j] = {it.lines > e->lines ? t.dev<uint64_t>(off_e) + it.ends : nullptr, it.lines - e->lines};
+            djobs[j] = df_job(z, it.need, it.last, ctx->h_dfout.as<uint8_t>() + out_at,
+                              (DfResumeResult*)(ctx->h_dfout.as<uint8_t>() + res_off) + j);
+            out_at += align_up(it.need.out, 256);
+            it.job = j++;
+        }
+        if (int rc = t.upload(ctx)) return rc;
+        if (nlines) {
+            filter_resume_kernel<<<(unsigned)((nlines + FILTER_WARPS - 1) / FILTER_WARPS), FILTER_WARPS * 32, 0, ctx->stream>>>(
+                t.dev<FilterResumeJob>(off_f), t.dev<uint32_t>(off_lb), (uint32_t)nfilter, (uint32_t)nlines);
+            ctx->launches++;
+            CU(cudaGetLastError());
+        }
+        // a non-interlaced encoder carries its last row to the next push (behind the filter launch, which reads the old one)
+        for (const Item& it : live) {
+            const pngb200_png_encoder* e = it.e;
+            if (e->interlaced || !it.d->n || it.last) continue;
+            const uint8_t* rows = it.d->memspace == PNGB200_MEM_HOST ? ctx->d_stin.as<uint8_t>() + it.staged : (const uint8_t*)it.d->rows;
+            CU(cudaMemcpyAsync(e->d_rows.p, rows + it.d->n - e->row_bytes, e->row_bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+        }
+        return PNGB200_OK;
+    };
+    if (int rc = enqueue()) {
+        for (Item& it : live) it.d->status = it.e->status = it.e->z->status = rc;
+        return rc;
+    }
+    cudaError_t err = cudaSuccess;
+    if (run) err = df_launch(ctx, t.dev<DfResumeJob>(off_dj), run, t.dev<DfEnds>(off_de));
+    else err = cudaStreamSynchronize(ctx->stream);
+    for (Item& it : live) {
+        pngb200_png_encoder* e = it.e;
+        int st = PNGB200_OK;
+        if (it.job != (size_t)-1) st = df_take(ctx, e->z, djobs[it.job], err);
+        else if (err != cudaSuccess) st = e->z->status = set_error(ctx, PNGB200_ERR_CUDA, "png_encoder: %s", cudaGetErrorString(err));
+        e->rows = it.rows, e->lines = it.lines;
+        it.d->status = e->status = st;
+    }
+    if (err != cudaSuccess) return PNGB200_ERR_CUDA;
+    // The IDAT CRC-32s: every new payload byte on the device, cut at chunk edges, the chunk type folded into a chunk's
+    // first piece; the stream header sits in d_header and the launch's bytes in d_out.
+    struct Piece { pngb200_png_encoder* e; uint64_t len; bool first; };
+    std::vector<CrcRegion> regions;
+    std::vector<Piece>     pieces;
+    for (Item& it : live) {
+        pngb200_png_encoder* e = it.e;
+        if (it.d->status != PNGB200_OK) continue;
+        const uint64_t chunk = e->z->chunk;
+        auto cut = [&](const uint8_t* p, uint64_t at, uint64_t len) {
+            while (len) {
+                const uint64_t take = std::min(len, (at / chunk + 1) * chunk - at);
+                regions.push_back({p, take, CK_IDAT, at % chunk == 0 ? 1u : 0u});
+                pieces.push_back({e, take, at % chunk == 0});
+                p += take, at += take, len -= take;
+            }
+        };
+        if (e->crc_at < e->header) cut(e->d_header.as<uint8_t>(), 0, e->header);
+        cut(e->z->d_out.as<uint8_t>(), it.written, e->z->written - it.written);
+    }
+    if (!regions.empty()) {
+        CrcPlan plan;
+        const uint32_t* crc = nullptr;
+        int rc = crc_upload(ctx, regions, nullptr, &plan);
+        if (rc == PNGB200_OK) rc = crc_launch(ctx, plan);
+        if (rc == PNGB200_OK) rc = crc_fetch(ctx, plan, &crc);
+        if (rc == PNGB200_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+            rc = set_error(ctx, PNGB200_ERR_CUDA, "png_encoder: CRC-32 pass failed");
+        if (rc != PNGB200_OK) {
+            for (const Piece& p : pieces) p.e->status = rc;
+            for (Item& it : live)
+                if (it.e->status != PNGB200_OK) it.d->status = it.e->status;
+            return rc;
+        }
+        for (size_t k = 0; k < pieces.size(); ++k) {
+            pngb200_png_encoder* e = pieces[k].e;
+            e->crc_open = pieces[k].first ? crc[k] : crc_combine(e->crc_open, crc[k], pieces[k].len);
+            e->crc_at += pieces[k].len;
+            if (e->crc_at % e->z->chunk == 0) e->crcs.push_back(e->crc_open);
+        }
+    }
+    // frame what the deflator hands out now: pop() before each scanline, then after the last push([], last: true)
+    // pull() until nil and IEND
+    for (Item& it : live) {
+        pngb200_png_encoder* e = it.e;
+        if (it.d->status != PNGB200_OK) continue;
+        pngb200_deflator* z = e->z;
+        if (z->finished && e->crc_at % z->chunk) e->crcs.push_back(e->crc_open);
+        const uint8_t* body;
+        size_t         n;
+        while (z->finished ? pngb200_deflator_pull(z, &body, &n) : pngb200_deflator_pop(z, &body, &n)) {
+            e->pieces.push_back(frame_idat(body, n, e->crcs.front()));
+            e->crcs.pop_front();
+        }
+        if (z->finished) {
+            std::vector<uint8_t> iend;
+            put_chunk(iend, CK_IEND, nullptr, 0);
+            e->pieces.push_back(std::move(iend));
+            e->iend = true;
+        }
+    }
+    return call.done();
+}
+
+}  // namespace
+
+extern "C" {
+
+pngb200_png_encoder* pngb200_png_encoder_create(pngb200_ctx* ctx, const pngb200_png_encoder_desc* d)
+{
+    Geometry g;
+    if (!ctx || !d || !encode_format_ok(d->format, d->width, d->height) || d->level < 0 || d->level > 13 ||
+        !geometry(d->width, d->height, d->format.depth * pixel_rule(d->format.color, d->format.depth, d->format.bgr).channels,
+                  d->format.depth, d->interlaced, &g)) {
+        set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_encoder_create: bad descriptor");
+        return nullptr;
+    }
+    // One push completes at most kMaxDeflatorPush filtered bytes.  A caller can always keep a non-interlaced push under
+    // that by pushing fewer rows, unless one scanline is over it; an Adam7 image's last row completes passes 1 to 6 at
+    // once (about 63/64 of its stream) whatever the schedule.  Such images are refused here, before any row is taken.
+    if (d->interlaced ? g.filtered > kMaxDeflatorPush : (uint64_t)g.pitch + 1 > kMaxDeflatorPush) {
+        set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_encoder_create: %s is over 1 GiB",
+                  d->interlaced ? "the filtered stream of an Adam7 image" : "a filtered scanline");
+        return nullptr;
+    }
+    const pngb200_pixel_format& f = d->format;
+    pngb200_png_encoder* e = new pngb200_png_encoder();
+    e->ctx = ctx;
+    e->width = d->width, e->height = d->height;
+    e->volume = (uint8_t)(f.depth * pixel_rule(f.color, f.depth, f.bgr).channels), e->depth = f.depth;
+    e->interlaced = d->interlaced ? 1 : 0, e->bpp = g.bpp;
+    e->row_bytes = (uint64_t)d->width * g.bpp;
+    e->z = pngb200_deflator_create_online(ctx, f.bgr ? PNGB200_FORMAT_IOS : PNGB200_FORMAT_ZLIB, d->level, 15,
+                                          d->idat_chunk ? d->idat_chunk : 65544);
+    if (!e->z) {
+        delete e;
+        return nullptr;
+    }
+    DeviceGuard guard(ctx->device);
+    e->header = e->z->output.size();
+    if (e->d_rows.reserve(e->interlaced ? g.storage : e->row_bytes) != cudaSuccess ||
+        e->d_header.reserve(std::max<uint64_t>(e->header, 1)) != cudaSuccess ||
+        (e->header && cudaMemcpy(e->d_header.p, e->z->output.data(), e->header, cudaMemcpyHostToDevice) != cudaSuccess) ||
+        ensure_crc_tables(ctx) != PNGB200_OK) {
+        set_error(ctx, PNGB200_ERR_CUDA, "png_encoder_create: cannot allocate the device state");
+        pngb200_deflator_destroy(e->z);
+        delete e;
+        return nullptr;
+    }
+    std::vector<uint8_t> head;
+    png_head(f, d->width, d->height, e->interlaced, head);
+    e->pieces.push_back(std::move(head));
+    return e;
+}
+
+void pngb200_png_encoder_destroy(pngb200_png_encoder* e)
+{
+    if (!e) return;
+    pngb200_deflator_destroy(e->z);   // synchronises the stream
+    DeviceGuard guard(e->ctx->device);
+    delete e;
+}
+
+int pngb200_png_encoder_push_batch(pngb200_ctx* ctx, pngb200_png_encoder_push_desc* pushes, size_t count)
+{
+    if (!ctx || (!pushes && count)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_encoder_push_batch: null argument");
+    std::vector<const void*> seen(count);
+    for (size_t i = 0; i < count; ++i) {
+        const pngb200_png_encoder* e = pushes[i].encoder;
+        if (!e || e->ctx != ctx || (!pushes[i].rows && pushes[i].n) ||
+            (pushes[i].memspace != PNGB200_MEM_HOST && pushes[i].memspace != PNGB200_MEM_DEVICE))
+            return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_encoder_push_batch: item %zu has no encoder of this context, "
+                             "no rows or no memspace", i);
+        seen[i] = e;
+    }
+    std::sort(seen.begin(), seen.end());
+    if (std::adjacent_find(seen.begin(), seen.end()) != seen.end())
+        return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "png_encoder_push_batch: a handle appears twice");
+    if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "a decode batch is pending");
+    if (!count) return PNGB200_OK;
+    DeviceGuard guard(ctx->device);
+    return encoder_pushes(ctx, pushes, count);
+}
+
+int pngb200_png_encoder_push(pngb200_png_encoder* e, const void* rows, size_t n, int memspace)
+{
+    if (!e) return PNGB200_ERR_BAD_ARGUMENT;
+    pngb200_png_encoder_push_desc d{e, rows, n, memspace, 0};
+    if (int rc = pngb200_png_encoder_push_batch(e->ctx, &d, 1)) return rc;
+    return d.status;
+}
+
+int pngb200_png_encoder_pop(pngb200_png_encoder* e, const uint8_t** bytes, size_t* n)
+{
+    if (!e || !bytes || !n) return PNGB200_ERR_BAD_ARGUMENT;
+    if (e->pieces.empty()) return 0;
+    e->popped = std::move(e->pieces.front());
+    e->pieces.pop_front();
+    const bool idat = e->popped.size() >= 8 && memcmp(e->popped.data() + 4, "IDAT", 4) == 0;
+    if (idat) e->idat_out++;
+    *bytes = e->popped.data();
+    *n = e->popped.size();
+    return 1;
+}
+
+int pngb200_png_encoder_progress(const pngb200_png_encoder* e, uint64_t out[6])
+{
+    if (!e || !out) return PNGB200_ERR_BAD_ARGUMENT;
+    out[0] = e->rows;
+    out[1] = e->lines;
+    out[2] = e->z->dequeued();
+    out[3] = e->idat_out;
+    out[4] = e->iend ? 1 : 0;
+    out[5] = e->device_bytes();
+    return PNGB200_OK;
+}
+
+void pngb200_png_encoder_error(const pngb200_png_encoder* e, int* status, uint32_t* a, uint32_t* b)
+{
+    if (status) *status = e ? e->status : PNGB200_ERR_BAD_ARGUMENT;
+    if (a) *a = 0;
+    if (b) *b = 0;
 }
 
 }  // extern "C"

@@ -9,9 +9,11 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <functional>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "checksum.cuh"
@@ -247,16 +249,27 @@ struct PushCall {
         list.clear();
         return PNGB200_OK;
     }
-    // Packs the items' bytes into the staging, uploads them with one copy and appends each item's at byte held() of
-    // its handle's d_in; `appended(d)` counts them in once that copy is queued.
+    // Packs the host byte ranges range(0 .. count - 1), each a (pointer, length) pair, back to back into the staging
+    // and uploads them with one copy: range k lands in d_stin behind the lengths of the ranges before it.
+    template <typename Range>
+    int pack(size_t count, Range range)
+    {
+        size_t off = 0;
+        for (size_t k = 0; k < count; ++k) {
+            const std::pair<const void*, size_t> r = range(k);
+            if (r.second) memcpy(ctx->h_stin.as<uint8_t>() + off, r.first, r.second), off += r.second;
+        }
+        if (off) CU(cudaMemcpyAsync(ctx->d_stin.p, ctx->h_stin.p, off, cudaMemcpyHostToDevice, ctx->stream));
+        return PNGB200_OK;
+    }
+    // Packs and uploads the items' bytes and appends each item's at byte held() of its handle's d_in; `appended(d)`
+    // counts them in once that copy is queued.
     template <typename Desc, typename Handle, typename Appended>
     int stage(const std::vector<Desc*>& items, Handle* Desc::*handle, Appended appended)
     {
+        if (int rc = pack(items.size(), [&](size_t k) { return std::pair<const void*, size_t>(items[k]->data, items[k]->n); }))
+            return rc;
         size_t off = 0;
-        for (const Desc* d : items)
-            if (d->n) memcpy(ctx->h_stin.as<uint8_t>() + off, d->data, d->n), off += d->n;
-        if (off) CU(cudaMemcpyAsync(ctx->d_stin.p, ctx->h_stin.p, off, cudaMemcpyHostToDevice, ctx->stream));
-        off = 0;
         for (Desc* d : items) {
             Handle* z = d->*handle;
             if (d->n)
@@ -1638,11 +1651,100 @@ void pngb200_deflator_destroy(pngb200_deflator* z)
 
 namespace {
 
+// The deflate side of a push call over online deflators, shared by pngb200_deflator_push_batch and
+// pngb200_png_encoder_push_batch.  What a handle needs for a push of n bytes: input from the base on; when it
+// compresses, a graph for every vertex the push can add to the unfinished block (full mode) and room for every byte
+// the launch can write.
+struct DfNeed { bool run; size_t in, graph, up, out; };
+constexpr uint64_t kMaxDeflatorPush = 1ull << 30;   // keeps every position of a launch inside int32
+
+DfNeed df_need(const pngb200_deflator* z, uint64_t n_new, bool last)
+{
+    const uint64_t total = z->total + n_new, n = total - z->base;
+    const uint64_t pending = total - z->dequeued();
+    DfNeed w;
+    w.run = pending > 4096 || last;   // DeflatorBuffers.swift:74, :120
+    w.in = n + 16;
+    w.graph = w.up = w.out = 0;
+    if (w.run) {
+        const bool full = z->level >= 8;
+        const uint64_t span = (uint64_t)((int64_t)n - z->end_index);
+        const uint64_t verts = std::min<uint64_t>(DF_GRAPH_CAP, (uint64_t)z->count + span) + 2;
+        if (full) w.graph = 128 * verts, w.up = 4 * (verts + 1);
+        w.out = pngb200_deflate_bound((full ? 1 : 8) * (uint64_t)z->count + span) + 4096;
+    }
+    return w;
+}
+
+// the buffers of `z` that `call` grows for `w`
+void df_grow(PushCall& call, pngb200_deflator* z, const DfNeed& w)
+{
+    if (w.in > z->d_in.cap) call.add(z->d_in, w.in, z->held());
+    if (w.graph > z->d_graph.cap) call.add(z->d_graph, w.graph, 128 * (size_t)z->count);
+    if (w.up > z->d_up.cap) call.add(z->d_up, w.up, 0);
+    if (w.out > z->d_out.cap) call.add(z->d_out, w.out, 0);
+}
+
+// the job of a handle that compresses, its new input counted in; its bytes and result land in pinned `host_dst` / `res`
+DfResumeJob df_job(pngb200_deflator* z, const DfNeed& w, bool last, uint8_t* host_dst, DfResumeResult* res)
+{
+    DfResumeJob j;
+    j.carry = z->d_carry.as<DfCarry>();
+    j.in = z->d_in.as<uint8_t>();
+    j.n = z->total - z->base;
+    j.dict = z->d_dict.as<int32_t>();
+    j.graph = z->d_graph.as<uint32_t>();
+    j.up = z->d_up.as<uint32_t>();
+    j.graph_vertices = z->d_graph.cap / 128;
+    j.dst = z->d_out.as<uint8_t>();
+    j.cap = w.out;
+    j.host_dst = host_dst;   // pinned: the kernel writes it over the bus (unified addressing)
+    j.result = res;
+    j.format = z->format;
+    j.level = z->level;
+    j.exponent = z->exponent;
+    j.last = last ? 1 : 0;
+    return j;
+}
+
+// one deflate_resume_kernel launch over `count` jobs already uploaded, then the synchronise
+cudaError_t df_launch(pngb200_ctx* ctx, const DfResumeJob* d_jobs, size_t count, const DfEnds* d_ends)
+{
+    deflate_resume_kernel<<<(unsigned)count, 32, sizeof(DfShared), ctx->stream>>>(d_jobs, (int)count, d_ends);
+    ctx->launches++;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    return e;
+}
+
+// takes a launched job's result into its handle (`e`: the launch's CUDA error); returns the item's status
+int df_take(pngb200_ctx* ctx, pngb200_deflator* z, const DfResumeJob& j, cudaError_t e)
+{
+    if (e != cudaSuccess)
+        return z->status = set_error(ctx, PNGB200_ERR_CUDA, "deflate_resume_kernel: %s", cudaGetErrorString(e));
+    const DfResumeResult& r = *j.result;
+    if (r.status != PNGB200_OK) return z->status = set_error(ctx, r.status, "deflate_resume_kernel: status %d", r.status);
+    z->output.insert(z->output.end(), j.host_dst, j.host_dst + r.produced);
+    z->blocks += r.blocks;
+    z->written += r.produced;
+    z->base = r.base;
+    z->end_index = r.end_index;
+    z->count = r.count;
+    if (j.last) z->finished = true;
+    return PNGB200_OK;
+}
+
+// what the reference's pop() handed out is gone from the queue
+void df_drop_popped(pngb200_deflator* z)
+{
+    z->output.erase(z->output.begin(), z->output.begin() + (ptrdiff_t)z->at);
+    z->at = 0;
+}
+
 // The pushes of one pngb200_deflator_push_batch call, on distinct online handles of `ctx`.  Every buffer the call
 // needs is allocated before any device work, so that an allocation failure leaves every handle as it was.
 int deflator_pushes(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t count)
 {
-    constexpr uint64_t kMaxPush = 1ull << 30;   // keeps every position of a launch inside int32
     std::vector<pngb200_deflator_push_desc*> live;
     size_t staged = 0;
     for (size_t i = 0; i < count; ++i) {
@@ -1650,31 +1752,14 @@ int deflator_pushes(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t
         pngb200_deflator* z = d->deflator;
         if (z->status < 0) d->status = z->status;
         else if (z->finished) d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "deflator: push after push(last: true)");
-        else if (d->n > kMaxPush) d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "deflator: a push is at most 1 GiB");
+        else if (d->n > kMaxDeflatorPush) d->status = set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "deflator: a push is at most 1 GiB");
         else d->status = PNGB200_ERR_CUDA, live.push_back(d), staged += d->n;   // until its push is answered
     }
-    // What each live item needs: input from the base on; when it compresses, a graph for every vertex the push can add
-    // to the unfinished block (full mode) and room for every byte the launch can write.
-    struct Need { bool run; size_t in, graph, up, out; };
-    std::vector<Need> need(live.size());
+    std::vector<DfNeed> need(live.size());
     size_t run = 0, host_out = 0;
     for (size_t k = 0; k < live.size(); ++k) {
-        const pngb200_deflator* z = live[k]->deflator;
-        const uint64_t total = z->total + live[k]->n, n = total - z->base;
-        const uint64_t pending = total - z->dequeued();
-        Need& w = need[k];
-        w.run = pending > 4096 || live[k]->last;   // DeflatorBuffers.swift:74, :120
-        w.in = n + 16;
-        w.graph = w.up = w.out = 0;
-        if (w.run) {
-            const bool full = z->level >= 8;
-            const uint64_t span = (uint64_t)((int64_t)n - z->end_index);
-            const uint64_t verts = std::min<uint64_t>(DF_GRAPH_CAP, (uint64_t)z->count + span) + 2;
-            if (full) w.graph = 128 * verts, w.up = 4 * (verts + 1);
-            w.out = pngb200_deflate_bound((full ? 1 : 8) * (uint64_t)z->count + span) + 4096;
-            host_out += align_up(w.out, 256);
-            run++;
-        }
+        need[k] = df_need(live[k]->deflator, live[k]->n, live[k]->last != 0);
+        if (need[k].run) host_out += align_up(need[k].out, 256), run++;
     }
     // every allocation, before any device work
     PushCall call(ctx);
@@ -1683,13 +1768,7 @@ int deflator_pushes(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t
     CU(ctx->h_dfout.reserve(res_off + sizeof(DfResumeResult) * std::max<size_t>(run, 1)));
     CU(ctx->h_st.reserve(jobs_bytes));
     CU(ctx->d_st.reserve(jobs_bytes));
-    for (size_t k = 0; k < live.size(); ++k) {
-        pngb200_deflator* z = live[k]->deflator;
-        if (need[k].in > z->d_in.cap) call.add(z->d_in, need[k].in, z->held());
-        if (need[k].graph > z->d_graph.cap) call.add(z->d_graph, need[k].graph, 128 * (size_t)z->count);
-        if (need[k].up > z->d_up.cap) call.add(z->d_up, need[k].up, 0);
-        if (need[k].out > z->d_out.cap) call.add(z->d_out, need[k].out, 0);
-    }
+    for (size_t k = 0; k < live.size(); ++k) df_grow(call, live[k]->deflator, need[k]);
     if (int rc = call.grow(staged)) return rc;
     // the new input of every handle with one upload, appended to its input
     if (int rc = call.stage(live, &pngb200_deflator_push_desc::deflator,
@@ -1701,65 +1780,22 @@ int deflator_pushes(pngb200_ctx* ctx, pngb200_deflator_push_desc* pushes, size_t
     for (size_t k = 0; k < live.size(); ++k) {
         pngb200_deflator_push_desc* d = live[k];
         pngb200_deflator* z = d->deflator;
-        // what the reference's pop() handed out is gone from the queue
-        z->output.erase(z->output.begin(), z->output.begin() + (ptrdiff_t)z->at);
-        z->at = 0;
+        df_drop_popped(z);
         if (!need[k].run) {
             d->status = PNGB200_OK;
             continue;
         }
-        DfResumeJob j;
-        j.carry = z->d_carry.as<DfCarry>();
-        j.in = z->d_in.as<uint8_t>();
-        j.n = z->total - z->base;
-        j.dict = z->d_dict.as<int32_t>();
-        j.graph = z->d_graph.as<uint32_t>();
-        j.up = z->d_up.as<uint32_t>();
-        j.graph_vertices = z->d_graph.cap / 128;
-        j.dst = z->d_out.as<uint8_t>();
-        j.cap = need[k].out;
-        j.host_dst = ctx->h_dfout.as<uint8_t>() + out_at;   // pinned: the kernel writes it over the bus (unified addressing)
-        j.result = (DfResumeResult*)(ctx->h_dfout.as<uint8_t>() + res_off) + jobs.size();
-        j.format = z->format;
-        j.level = z->level;
-        j.exponent = z->exponent;
-        j.last = d->last ? 1 : 0;
+        jobs.push_back(df_job(z, need[k], d->last != 0, ctx->h_dfout.as<uint8_t>() + out_at,
+                              (DfResumeResult*)(ctx->h_dfout.as<uint8_t>() + res_off) + jobs.size()));
         out_at += align_up(need[k].out, 256);
-        jobs.push_back(j);
         which.push_back(k);
     }
     if (!jobs.empty()) {
         memcpy(ctx->h_st.p, jobs.data(), sizeof(DfResumeJob) * jobs.size());
         cudaError_t e = cudaMemcpyAsync(ctx->d_st.p, ctx->h_st.p, sizeof(DfResumeJob) * jobs.size(), cudaMemcpyHostToDevice,
                                         ctx->stream);
-        if (e == cudaSuccess) {
-            deflate_resume_kernel<<<(unsigned)jobs.size(), 32, sizeof(DfShared), ctx->stream>>>(ctx->d_st.as<DfResumeJob>(),
-                                                                                                 (int)jobs.size());
-            ctx->launches++;
-            e = cudaGetLastError();
-        }
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-        for (size_t t = 0; t < jobs.size(); ++t) {
-            pngb200_deflator_push_desc* d = live[which[t]];
-            pngb200_deflator* z = d->deflator;
-            if (e != cudaSuccess) {
-                z->status = d->status = set_error(ctx, PNGB200_ERR_CUDA, "deflate_resume_kernel: %s", cudaGetErrorString(e));
-                continue;
-            }
-            const DfResumeResult& r = *jobs[t].result;
-            d->status = r.status;
-            if (r.status != PNGB200_OK) {
-                z->status = set_error(ctx, r.status, "deflate_resume_kernel: status %d", r.status);
-                continue;
-            }
-            z->output.insert(z->output.end(), jobs[t].host_dst, jobs[t].host_dst + r.produced);
-            z->blocks += r.blocks;
-            z->written += r.produced;
-            z->base = r.base;
-            z->end_index = r.end_index;
-            z->count = r.count;
-            if (d->last) z->finished = true;
-        }
+        if (e == cudaSuccess) e = df_launch(ctx, ctx->d_st.as<DfResumeJob>(), jobs.size(), nullptr);
+        for (size_t t = 0; t < jobs.size(); ++t) live[which[t]]->status = df_take(ctx, live[which[t]]->deflator, jobs[t], e);
         if (e != cudaSuccess) return PNGB200_ERR_CUDA;
     } else if (staged) {
         if (cudaStreamSynchronize(ctx->stream) != cudaSuccess)
