@@ -647,6 +647,52 @@ int  pngb200_png_encoder_progress(const pngb200_png_encoder* e, uint64_t out[6])
 /* the sticky device error (PNGB200_OK if none); a and b are 0 (kept for the shape of the other handles' calls) */
 void pngb200_png_encoder_error(const pngb200_png_encoder* e, int* status, uint32_t* a, uint32_t* b);
 
+/* ---- cloning handles: LZ77.Inflator, LZ77.Deflator, PNG.Context and PNG.Encoder are values ----------------------------
+ * In the reference these types are structs whose buffers are copied on write (exclude(), LZ77.InflatorBuffers.swift,
+ * LZ77.DeflatorIn.swift, LZ77.DeflatorOut.swift), so after `var b = a` a push into `a` never changes `b`.  A clone is
+ * that copy, made eagerly: a new handle of the source's type on the same ctx, with its own device buffers.
+ * The contract: take a clone made from source S and any later sequence of calls on it.  Each call returns exactly what
+ * the same call on S would have returned at the moment of cloning: statuses and error payloads, available / pull /
+ * pull_all, pop and pull blocks, progress (all six values of a context, the band included), storage bytes, encoder
+ * pieces and stats() -- except the device bytes a handle holds (pngb200_deflator_stats out[3],
+ * pngb200_png_encoder_progress out[5]): a clone holds no launch scratch and only the bytes in use, so right after the
+ * clone it holds at most what the source holds, and later pushes grow it from there.  After the clone,
+ * no call on either handle changes anything the other returns.  This holds for terminal handles, handles with a sticky
+ * error (the clone keeps it), deflators after `last`, and encoders with pieces not yet popped (each handle pops its own
+ * copy).  A context clone's storage starts as the bytes of the source's storage; `pixels` must stay valid while the
+ * clone lives, as the storage given to pngb200_png_context_create.
+ * Rejections, PNGB200_ERR_BAD_ARGUMENT before any work with every `clone` left NULL: a null ctx, or a null array with
+ * count > 0; an item whose number of non-null source fields is not exactly one; a source of another ctx; a context
+ * item with null `pixels`, a `pixels_cap` below the source's storage bytes, or storage bytes at `pixels` that overlap
+ * the source's storage; a call while a decode batch is pending on the ctx.  The same source may appear twice: it gets
+ * two clones.
+ * All or nothing: if an allocation or a copy fails the call returns PNGB200_ERR_CUDA, every clone it made is destroyed
+ * (each `clone` NULL) and every source is unchanged.
+ * Fixed cost, whatever `count`: one upload of the copy list, at most one segment_copy_kernel launch (every source's
+ * device bytes in use, into freshly allocated buffers) and one stream synchronise.  Host state (queues, tails, a
+ * buffered deflator's input, host storage) is copied on the host; a call whose items hold no device bytes (fresh
+ * handles, buffered deflators) makes no launch.  A clone's device buffers are those create gives a handle, plus the
+ * bytes in use of the buffers pushes grow (an inflator's output keeps the source's capacity, which decides when the
+ * decoder stops to grow it); the next push grows them as it would on any handle. */
+typedef struct pngb200_clone_desc {
+    pngb200_inflator*    inflator;
+    pngb200_deflator*    deflator;     /* online or buffered */
+    pngb200_png_context* context;
+    pngb200_png_encoder* encoder;
+    void*                pixels;       /* context only: the clone's storage, in the source's memspace, any alignment */
+    size_t               pixels_cap;   /* >= the source's storage bytes */
+    void*                clone;        /* out: a handle of the source's type on the same ctx */
+} pngb200_clone_desc;
+int pngb200_clone_batch(pngb200_ctx* ctx, pngb200_clone_desc* items, size_t count);
+/* the bytes the last successful pngb200_clone_batch on `ctx` copied: out[0] device bytes (its one launch), out[1] host
+ * bytes (queues, tails, buffered input, host storage); both 0 after a call that failed */
+int pngb200_ctx_clone_stats(pngb200_ctx* ctx, uint64_t out[2]);
+/* pngb200_clone_batch with one item: the clone, or NULL with the reason in pngb200_last_error */
+pngb200_inflator*    pngb200_inflator_clone(const pngb200_inflator* z);
+pngb200_deflator*    pngb200_deflator_clone(const pngb200_deflator* z);
+pngb200_png_context* pngb200_png_context_clone(const pngb200_png_context* c, void* pixels, size_t pixels_cap);
+pngb200_png_encoder* pngb200_png_encoder_clone(const pngb200_png_encoder* e);
+
 #ifdef __cplusplus
 }
 #endif

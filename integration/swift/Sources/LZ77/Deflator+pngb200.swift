@@ -21,6 +21,11 @@ extension LZ77
                 // when the reference would
                 self.z = pngb200_deflator_create_online(LZ77.GPU.shared.ctx, format, Int32.init(level), Int32.init(exponent), chunk)!
             }
+            /// A copy of `other` on the device that goes on independently (pngb200_deflator_clone).
+            init(cloning other:Handle)
+            {
+                self.z = pngb200_deflator_clone(other.z)!
+            }
             deinit
             {
                 pngb200_deflator_destroy(self.z)
@@ -28,6 +33,17 @@ extension LZ77
         }
         private
         var handle:Handle
+
+        /// What `exclude()` does (LZ77.DeflatorIn.swift, LZ77.DeflatorOut.swift): a shared handle is cloned before it
+        /// is written.
+        fileprivate mutating
+        func exclude()
+        {
+            if !isKnownUniquelyReferenced(&self.handle)
+            {
+                self.handle = .init(cloning: self.handle)
+            }
+        }
 
         public
         init(format:LZ77.Format = .zlib, level:Int, exponent:Int = 15, hint:Int = 1 << 12)
@@ -41,6 +57,7 @@ extension LZ77.Deflator
     public mutating
     func push(_ data:ArraySlice<UInt8>, last:Bool = false)
     {
+        self.exclude()
         let status:Int32 = data.withUnsafeBufferPointer
         {
             pngb200_deflator_push(self.handle.z, $0.baseAddress, $0.count, last ? 1 : 0)
@@ -51,6 +68,7 @@ extension LZ77.Deflator
     public mutating
     func pull() -> [UInt8]?
     {
+        self.exclude()
         var block:UnsafePointer<UInt8>? = nil, count:Int = 0
         return pngb200_deflator_pull(self.handle.z, &block, &count) == 1
             ? .init(UnsafeBufferPointer.init(start: block, count: count)) : nil
@@ -59,6 +77,7 @@ extension LZ77.Deflator
     public mutating
     func pop() -> [UInt8]?
     {
+        self.exclude()
         var block:UnsafePointer<UInt8>? = nil, count:Int = 0
         return pngb200_deflator_pop(self.handle.z, &block, &count) == 1
             ? .init(UnsafeBufferPointer.init(start: block, count: count)) : nil

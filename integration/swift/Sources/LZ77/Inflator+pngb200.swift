@@ -15,6 +15,11 @@ extension LZ77
             {
                 self.z = pngb200_inflator_create(LZ77.GPU.shared.ctx, format)!
             }
+            /// A copy of `other` on the device that goes on independently (pngb200_inflator_clone).
+            init(cloning other:Handle)
+            {
+                self.z = pngb200_inflator_clone(other.z)!
+            }
             deinit
             {
                 pngb200_inflator_destroy(self.z)
@@ -22,6 +27,16 @@ extension LZ77
         }
         private
         var handle:Handle
+
+        /// What `exclude()` does (LZ77.InflatorBuffers.swift): a shared handle is cloned before it is written.
+        fileprivate mutating
+        func exclude()
+        {
+            if !isKnownUniquelyReferenced(&self.handle)
+            {
+                self.handle = .init(cloning: self.handle)
+            }
+        }
 
         public
         init(format:LZ77.Format = .zlib)
@@ -36,6 +51,7 @@ extension LZ77.Inflator
     public mutating
     func push(_ data:ArraySlice<UInt8>) throws -> Void?
     {
+        self.exclude()
         let status:Int32 = data.withUnsafeBufferPointer
         {
             pngb200_inflator_push(self.handle.z, $0.baseAddress, $0.count)
@@ -54,12 +70,14 @@ extension LZ77.Inflator
     public mutating
     func pull(_ count:Int) -> [UInt8]?
     {
+        self.exclude()
         var out:[UInt8] = .init(repeating: 0, count: count)
         return pngb200_inflator_pull(self.handle.z, &out, count) == 0 ? out : nil
     }
     public mutating
     func pull() -> [UInt8]
     {
+        self.exclude()
         var out:[UInt8] = .init(repeating: 0, count: pngb200_inflator_available(self.handle.z))
         let n:Int = pngb200_inflator_pull_all(self.handle.z, &out, out.count)
         out.removeLast(out.count - n)

@@ -124,5 +124,30 @@ extension PNG
             pngb200_png_context_destroy(self.handle)
             self.storage.deallocate()
         }
+
+        private
+        init(handle:OpaquePointer, storage:UnsafeMutableBufferPointer<UInt8>)
+        {
+            self.handle = handle
+            self.storage = storage
+        }
+        /// An independent copy (pngb200_png_context_clone), its storage starting as this one's.  `storage`, of at least
+        /// this context's storage bytes, becomes the copy's and is deallocated by its `destroy()`; nil allocates it.
+        /// On failure (nil) a caller's `storage` stays the caller's.  The copy has a lifetime of its own: destroy both.
+        func copy(storage given:UnsafeMutableBufferPointer<UInt8>? = nil) -> Self?
+        {
+            let storage:UnsafeMutableBufferPointer<UInt8> = given ?? .allocate(capacity: self.storage.count)
+            guard let handle:OpaquePointer = pngb200_png_context_clone(self.handle,
+                UnsafeMutableRawPointer.init(storage.baseAddress), storage.count)
+            else
+            {
+                if  given == nil
+                {
+                    storage.deallocate()
+                }
+                return nil
+            }
+            return .init(handle: handle, storage: storage)
+        }
     }
 }

@@ -93,6 +93,24 @@ extension PNG
         {
             pngb200_png_encoder_destroy(self.handle)
         }
+
+        private
+        init(handle:OpaquePointer, stride:Int)
+        {
+            self.handle = handle
+            self.stride = stride
+        }
+        /// An independent copy (pngb200_png_encoder_clone) with its own copy of the pieces not popped yet.  The copy has
+        /// a lifetime of its own: destroy both.
+        func copy() -> Self?
+        {
+            guard let handle:OpaquePointer = pngb200_png_encoder_clone(self.handle)
+            else
+            {
+                return nil
+            }
+            return .init(handle: handle, stride: self.stride)
+        }
     }
 }
 

@@ -202,6 +202,11 @@ class PngEncoderPushDesc(C.Structure):
                 ("status", C.c_int32)]
 
 
+class CloneDesc(C.Structure):
+    _fields_ = [("inflator", C.c_void_p), ("deflator", C.c_void_p), ("context", C.c_void_p), ("encoder", C.c_void_p),
+                ("pixels", C.c_void_p), ("pixels_cap", C.c_size_t), ("clone", C.c_void_p)]
+
+
 class PNGB200Error(RuntimeError):
     def __init__(self, status: int, message: str = ""):
         super().__init__(f"pngb200 status {status}: {message}")
@@ -369,6 +374,16 @@ def lib():
         L.pngb200_png_encoder_error.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_uint32),
                                                 C.POINTER(C.c_uint32)]
         L.pngb200_png_encoder_error.restype = None
+    if hasattr(L, "pngb200_clone_batch"):
+        L.pngb200_clone_batch.argtypes = [C.c_void_p, C.POINTER(CloneDesc), C.c_size_t]
+        L.pngb200_clone_batch.restype = C.c_int
+        for name in ("inflator", "deflator", "png_encoder"):
+            getattr(L, f"pngb200_{name}_clone").argtypes = [C.c_void_p]
+            getattr(L, f"pngb200_{name}_clone").restype = C.c_void_p
+        L.pngb200_png_context_clone.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        L.pngb200_png_context_clone.restype = C.c_void_p
+        L.pngb200_ctx_clone_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.pngb200_ctx_clone_stats.restype = C.c_int
     _lib = L
     return L
 
@@ -459,6 +474,12 @@ class Context:
         out = (C.c_uint64 * 3)()
         self.check(self._lib.pngb200_ctx_unfilter_stats(self.handle, out))
         return dict(wavefront=out[0], passes=out[1], generic=out[2])
+
+    def clone_stats(self):
+        """(device bytes, host bytes) the last clone_batch on this context copied (see pngb200_ctx_clone_stats)"""
+        out = (C.c_uint64 * 2)()
+        self.check(self._lib.pngb200_ctx_clone_stats(self.handle, out))
+        return out[0], out[1]
 
     def split_stats(self):
         """bytes and SM cycles of the heads and tails of the streams the last batch cut in two, the tails that left
@@ -909,6 +930,10 @@ class Deflator:
         self.ctx.check(self.ctx._lib.pngb200_deflator_stats(self.handle, out))
         return tuple(out)
 
+    def clone(self) -> "Deflator":
+        """a copy that goes on independently (Swift: `var b = a`)"""
+        return clone_batch(self.ctx, [self])[0]
+
 
 class Inflator:
     """LZ77.Inflator / Gzip.Inflator value semantics over the GPU path (streaming push/pull)."""
@@ -964,6 +989,10 @@ class Inflator:
         if st != OK:
             raise PNGB200Error(st, "inflator_stats")
         return {"bits": out[0], "bytes": out[1], "serial_bytes": out[2]}
+
+    def clone(self) -> "Inflator":
+        """a copy that goes on independently (Swift: `var b = a`)"""
+        return clone_batch(self.ctx, [self])[0]
 
 
 class PngContext:
@@ -1027,6 +1056,11 @@ class PngContext:
         """host storage: its bytes; device storage: its address"""
         return C.string_at(self._addr, self._size) if self._host is not None else self._addr
 
+    def clone(self, pixels=None) -> "PngContext":
+        """a copy that goes on independently, its storage starting as this one's.  `pixels`: None for new storage in
+        this context's memspace (host bytes, or a device buffer the clone owns), or a device buffer (address, length)
+        apart from this one's storage for a context with device storage"""
+        return clone_batch(self.ctx, [(self, pixels)])[0]
 
 
 def _push_batch(ctx: Context, kind, entry, items):
@@ -1122,6 +1156,10 @@ class PngEncoder:
         self.ctx._lib.pngb200_png_encoder_error(self.handle, C.byref(s), C.byref(a), C.byref(b))
         return s.value
 
+    def clone(self) -> "PngEncoder":
+        """a copy that goes on independently, with its own copy of the pieces not popped yet"""
+        return clone_batch(self.ctx, [self])[0]
+
 
 def png_encoder_push_batch(ctx: Context, items) -> list:
     """pushes of many PngEncoders in one call: `items` is [(encoder, rows[, memspace])], distinct encoders of `ctx`,
@@ -1140,3 +1178,41 @@ def png_encoder_push_batch(ctx: Context, items) -> list:
             d.rows, d.n = C.cast(C.c_char_p(data), C.c_void_p), len(data)
     ctx.check(ctx._lib.pngb200_png_encoder_push_batch(ctx.handle, descs, len(items)))
     return [descs[i].status for i in range(len(items))]
+
+
+def clone_batch(ctx: Context, items) -> list:
+    """Clone many handles in one call (pngb200_clone_batch): `items` holds Inflators, Deflators, PngEncoders and
+    PngContexts, a context optionally as (png_context, pixels) with `pixels` as PngContext.clone takes it.  Returns the
+    clones in order; raises PNGB200Error, with no clone made, when the call fails."""
+    descs = (CloneDesc * max(len(items), 1))()
+    field = {Inflator: "inflator", Deflator: "deflator", PngContext: "context", PngEncoder: "encoder"}
+    storage = []   # per context item: (host buffer, device tensor, address)
+    for d, item in zip(descs, items):
+        src, pixels = item if isinstance(item, tuple) else (item, None)
+        setattr(d, field[type(src)], src.handle)
+        if isinstance(src, PngContext):
+            host, dev = None, None
+            if pixels is not None and src._host is not None:
+                raise PNGB200Error(ERR_BAD_ARGUMENT, "clone_batch: a context with host storage takes no pixels")
+            if pixels is not None:
+                addr, cap = pixels
+            elif src._host is not None:
+                host = C.create_string_buffer(max(src._size, 1))
+                addr, cap = C.addressof(host), src._size
+            else:
+                import torch
+                dev = torch.empty(max(src._size, 1), dtype=torch.uint8, device=f"cuda:{ctx.device}")
+                addr, cap = dev.data_ptr(), src._size
+            d.pixels, d.pixels_cap = addr, cap
+            storage.append((host, dev, addr))
+    ctx.check(ctx._lib.pngb200_clone_batch(ctx.handle, descs, len(items)))
+    out, k = [], 0
+    for d, item in zip(descs, items):
+        src = item[0] if isinstance(item, tuple) else item
+        c = type(src).__new__(type(src))
+        c.ctx, c.handle = src.ctx, d.clone
+        if isinstance(src, PngContext):
+            c._size, (c._host, c._dev, c._addr) = src._size, storage[k]
+            k += 1
+        out.append(c)
+    return out

@@ -1107,3 +1107,161 @@ void pngb200_png_encoder_error(const pngb200_png_encoder* e, int* status, uint32
 }
 
 }  // extern "C"
+
+// ---------------- cloning handles: the encoder and pngb200_clone_batch ----------------
+namespace {
+
+cudaError_t clone_encoder(const pngb200_png_encoder* s, pngb200_png_encoder* e, std::vector<CopySegment>& segs)
+{
+    e->ctx = s->ctx;
+    e->width = s->width, e->height = s->height;
+    e->volume = s->volume, e->depth = s->depth, e->interlaced = s->interlaced, e->bpp = s->bpp;
+    e->row_bytes = s->row_bytes, e->rows = s->rows, e->lines = s->lines;
+    e->header = s->header;
+    e->status = s->status;
+    e->crc_at = s->crc_at, e->crc_open = s->crc_open, e->crcs = s->crcs;
+    e->pieces = s->pieces;   // each handle pops its own copy; `popped` starts empty
+    e->idat_out = s->idat_out, e->iend = s->iend;
+    e->z = new pngb200_deflator();
+    cudaError_t err = clone_deflator(s->z, e->z, segs);
+    // Adam7: the whole storage, of which the rows received are written; otherwise the row carried to the next push
+    const uint64_t rows = e->interlaced ? s->row_bytes * s->height : s->row_bytes;
+    const uint64_t keep = e->interlaced ? s->row_bytes * s->rows : s->rows ? s->row_bytes : 0;
+    if (err == cudaSuccess) err = clone_buf(segs, e->d_rows, s->d_rows, rows, keep, false);
+    if (err == cudaSuccess) err = clone_buf(segs, e->d_header, s->d_header, std::max<uint64_t>(s->header, 1), s->header, false);
+    return err;
+}
+
+// the host bytes an item's clone copies: queues, tails, a buffered deflator's input, host storage
+uint64_t clone_host_bytes(const pngb200_clone_desc& d)
+{
+    auto deflator = [](const pngb200_deflator* z) { return (uint64_t)(z->input.size() + z->output.size()); };
+    if (d.inflator) return d.inflator->tail.size();
+    if (d.deflator) return deflator(d.deflator);
+    if (d.context) return d.context->z->tail.size() + (d.context->memspace == PNGB200_MEM_HOST ? d.context->storage : 0);
+    uint64_t n = deflator(d.encoder->z) + sizeof(uint32_t) * d.encoder->crcs.size();
+    for (const std::vector<uint8_t>& piece : d.encoder->pieces) n += piece.size();
+    return n;
+}
+
+void destroy_clone(pngb200_clone_desc& d)
+{
+    if (!d.clone) return;
+    if (d.inflator) pngb200_inflator_destroy((pngb200_inflator*)d.clone);
+    else if (d.deflator) pngb200_deflator_destroy((pngb200_deflator*)d.clone);
+    else if (d.context) pngb200_png_context_destroy((pngb200_png_context*)d.clone);
+    else pngb200_png_encoder_destroy((pngb200_png_encoder*)d.clone);
+    d.clone = nullptr;
+}
+
+// The checks of pngb200_clone_batch, made before any work
+int check_clones(pngb200_ctx* ctx, const pngb200_clone_desc* items, size_t count)
+{
+    if (!ctx || (!items && count)) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "clone_batch: null argument");
+    for (size_t i = 0; i < count; ++i) {
+        const pngb200_clone_desc& d = items[i];
+        const int sources = !!d.inflator + !!d.deflator + !!d.context + !!d.encoder;
+        const pngb200_ctx* owner = d.inflator ? d.inflator->ctx : d.deflator ? d.deflator->ctx : d.context ? d.context->ctx
+                                 : d.encoder ? d.encoder->ctx : nullptr;
+        if (sources != 1 || owner != ctx)
+            return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "clone_batch: item %zu has not exactly one source of this context", i);
+        if (d.context) {
+            const uintptr_t a = (uintptr_t)d.pixels, b = (uintptr_t)d.context->pixels, n = (uintptr_t)d.context->storage;
+            if (!d.pixels || d.pixels_cap < d.context->storage || (n && a < b + n && b < a + n))
+                return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "clone_batch: item %zu has no storage of %llu bytes apart from its "
+                                 "source's", i, (unsigned long long)n);
+        }
+    }
+    if (ctx->pending) return set_error(ctx, PNGB200_ERR_BAD_ARGUMENT, "clone_batch: a decode batch is pending");
+    return PNGB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pngb200_clone_batch(pngb200_ctx* ctx, pngb200_clone_desc* items, size_t count)
+{
+    for (size_t i = 0; items && i < count; ++i) items[i].clone = nullptr;
+    if (ctx) ctx->clone_bytes[0] = ctx->clone_bytes[1] = 0;
+    if (int rc = check_clones(ctx, items, count)) return rc;
+    if (!count) return PNGB200_OK;
+    DeviceGuard guard(ctx->device);
+    std::vector<CopySegment> segs;
+    cudaError_t e = cudaSuccess;
+    for (size_t i = 0; i < count && e == cudaSuccess; ++i) {
+        pngb200_clone_desc& d = items[i];
+        if (d.inflator) {
+            pngb200_inflator* z = new pngb200_inflator();
+            d.clone = z;
+            e = clone_inflator(d.inflator, z, segs);
+        } else if (d.deflator) {
+            pngb200_deflator* z = new pngb200_deflator();
+            d.clone = z;
+            e = clone_deflator(d.deflator, z, segs);
+        } else if (d.context) {
+            pngb200_png_context* c = new pngb200_png_context();
+            d.clone = c;
+            e = clone_context(d.context, c, (uint8_t*)d.pixels, segs);
+        } else {
+            pngb200_png_encoder* c = new pngb200_png_encoder();
+            d.clone = c;
+            e = clone_encoder(d.encoder, c, segs);
+        }
+    }
+    int rc = e == cudaSuccess ? PNGB200_OK
+                              : set_error(ctx, PNGB200_ERR_CUDA, "clone_batch: cannot allocate a clone: %s", cudaGetErrorString(e));
+    // One launch copies every segment.  Each starts at byte 0 of a DevBuf, which cudaMalloc aligns, so the kernel's
+    // misaligned branch never runs for them -- except a context's device storage, at the caller's alignment: there the
+    // last word that branch reads is the aligned word holding the segment's last byte, inside the same allocation.
+    if (rc == PNGB200_OK && !segs.empty()) {
+        CopyPlan plan;
+        rc = copy_upload(ctx, segs, &plan);
+        if (rc == PNGB200_OK) rc = copy_launch(ctx, plan);
+        if (rc == PNGB200_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess)
+            rc = set_error(ctx, PNGB200_ERR_CUDA, "clone_batch: the copy failed");
+    }
+    if (rc != PNGB200_OK) {
+        for (size_t i = 0; i < count; ++i) destroy_clone(items[i]);
+        return rc;
+    }
+    for (size_t i = 0; i < count; ++i) {
+        if (items[i].context && items[i].context->memspace == PNGB200_MEM_HOST)
+            memcpy(items[i].pixels, items[i].context->pixels, items[i].context->storage);
+        ctx->clone_bytes[1] += clone_host_bytes(items[i]);
+    }
+    for (const CopySegment& s : segs) ctx->clone_bytes[0] += s.len;
+    return PNGB200_OK;
+}
+
+pngb200_inflator* pngb200_inflator_clone(const pngb200_inflator* z)
+{
+    pngb200_clone_desc d{};
+    d.inflator = const_cast<pngb200_inflator*>(z);
+    return pngb200_clone_batch(z ? z->ctx : nullptr, &d, 1) ? nullptr : (pngb200_inflator*)d.clone;
+}
+
+pngb200_deflator* pngb200_deflator_clone(const pngb200_deflator* z)
+{
+    pngb200_clone_desc d{};
+    d.deflator = const_cast<pngb200_deflator*>(z);
+    return pngb200_clone_batch(z ? z->ctx : nullptr, &d, 1) ? nullptr : (pngb200_deflator*)d.clone;
+}
+
+pngb200_png_context* pngb200_png_context_clone(const pngb200_png_context* c, void* pixels, size_t pixels_cap)
+{
+    pngb200_clone_desc d{};
+    d.context = const_cast<pngb200_png_context*>(c);
+    d.pixels = pixels;
+    d.pixels_cap = pixels_cap;
+    return pngb200_clone_batch(c ? c->ctx : nullptr, &d, 1) ? nullptr : (pngb200_png_context*)d.clone;
+}
+
+pngb200_png_encoder* pngb200_png_encoder_clone(const pngb200_png_encoder* e)
+{
+    pngb200_clone_desc d{};
+    d.encoder = const_cast<pngb200_png_encoder*>(e);
+    return pngb200_clone_batch(e ? e->ctx : nullptr, &d, 1) ? nullptr : (pngb200_png_encoder*)d.clone;
+}
+
+}  // extern "C"

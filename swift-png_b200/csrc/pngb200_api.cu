@@ -121,6 +121,7 @@ struct pngb200_ctx {
     PinBuf h_dfout;   // the online deflators' launch: the bytes each handle wrote and its result, written by the kernel
     uint64_t seg_streams = 0, seg_segments = 0, seg_fallbacks = 0;  // last batch: streams cut into segments, segments, rejected
     uint64_t split_stats[6] = {};      // last batch, streams cut in two: see pngb200_ctx_split_stats
+    uint64_t clone_bytes[2] = {};      // last pngb200_clone_batch: device bytes, host bytes copied
     uint64_t scratch_stride = 0;       // layout of d_scratch the last inflate launch used
     size_t parallel_threshold = 8192;  // streams at least this long use the block-parallel kernel
     unsigned long long* d_hist = nullptr;   // filter-type histogram of the last wavefront-unfilter launch (in d_imgjobs)
@@ -1218,6 +1219,14 @@ int pngb200_ctx_split_stats(pngb200_ctx* ctx, uint64_t out[6])
 {
     if (!ctx || !out) return PNGB200_ERR_BAD_ARGUMENT;
     for (int k = 0; k < 6; ++k) out[k] = ctx->split_stats[k];
+    return PNGB200_OK;
+}
+
+int pngb200_ctx_clone_stats(pngb200_ctx* ctx, uint64_t out[2])
+{
+    if (!ctx || !out) return PNGB200_ERR_BAD_ARGUMENT;
+    out[0] = ctx->clone_bytes[0];
+    out[1] = ctx->clone_bytes[1];
     return PNGB200_OK;
 }
 
@@ -2736,5 +2745,96 @@ void pngb200_png_context_error(const pngb200_png_context* c, int* status, uint32
 }
 
 }  // extern "C"
+
+// ---------------- cloning handles (pngb200_clone_batch) ----------------
+// A clone routine fills a new handle from its source: host state by assignment, and for each device buffer a fresh
+// allocation plus a CopySegment for the bytes in use, which the call copies for every item with one launch.  The
+// carried device state holds positions, not addresses (DfCarry is relative to its base, ResumePoint counts bits and
+// bytes, and every launch builds its DfResumeJob / StreamJob pointers anew), so copied bytes are a valid state.  A
+// routine that fails leaves what it allocated in the new handle, which the caller destroys.
+namespace {
+
+// `dst` takes `size` bytes: as create reserves them (`exact` false: a buffer fixed at create that later pushes write
+// without a reserve), or exactly (a buffer pushes grow, given only its bytes in use); `src`'s first `keep` bytes are
+// queued for the copy.
+cudaError_t clone_buf(std::vector<CopySegment>& segs, DevBuf& dst, const DevBuf& src, size_t size, size_t keep, bool exact)
+{
+    if (!size) return cudaSuccess;
+    cudaError_t e;
+    if (exact) {
+        e = cudaMalloc(&dst.p, size);
+        if (e == cudaSuccess) dst.cap = size;
+    } else {
+        e = dst.reserve(size);
+    }
+    if (e == cudaSuccess && keep) segs.push_back({src.as<uint8_t>(), dst.as<uint8_t>(), (uint64_t)keep});
+    return e;
+}
+
+cudaError_t clone_inflator(const pngb200_inflator* s, pngb200_inflator* z, std::vector<CopySegment>& segs)
+{
+    z->ctx = s->ctx;
+    z->format = s->format;
+    z->pushed = s->pushed, z->tail_at = s->tail_at, z->tail = s->tail;
+    z->resume_bit = s->resume_bit, z->resume_out = s->resume_out, z->produced = s->produced, z->current = s->current;
+    z->phase = s->phase;
+    z->at = s->at;
+    for (int k = 0; k < 3; ++k) z->work[k] = s->work[k];
+    z->terminal = s->terminal;
+    z->status = s->status, z->err_a = s->err_a, z->err_b = s->err_b;
+    // every byte pushed, with the bit reader's 16 bytes of slack
+    cudaError_t e = clone_buf(segs, z->d_in, s->d_in, s->pushed ? s->pushed + 16 : 0, s->pushed, true);
+    // Pulls read the output from `current` and a resumed launch reads the window behind `produced`.  The output keeps
+    // the source's capacity: a launch that runs out of it stops for another round, which decodes bits again and so
+    // shows in stats(), so a smaller buffer would make the clone's stats differ from its source's.
+    if (e == cudaSuccess) e = clone_buf(segs, z->d_out, s->d_out, s->d_out.cap, s->produced, true);
+    return e;
+}
+
+cudaError_t clone_deflator(const pngb200_deflator* s, pngb200_deflator* z, std::vector<CopySegment>& segs)
+{
+    z->ctx = s->ctx;
+    z->format = s->format, z->level = s->level, z->exponent = s->exponent;
+    z->chunk = s->chunk;
+    z->input = s->input, z->output = s->output, z->at = s->at;
+    z->finished = s->finished;
+    z->online = s->online;
+    z->status = s->status;
+    z->total = s->total, z->base = s->base, z->end_index = s->end_index, z->count = s->count;
+    z->blocks = s->blocks, z->written = s->written;
+    if (!s->online) return cudaSuccess;
+    // d_up is scratch of one launch and d_out's bytes reach the host (or the encoder's CRC step) within the call that
+    // writes them: neither is carried.  The graph keeps the unfinished block's vertices, as df_grow does.
+    cudaError_t e = clone_buf(segs, z->d_carry, s->d_carry, sizeof(DfCarry), sizeof(DfCarry), false);
+    if (e == cudaSuccess) e = clone_buf(segs, z->d_dict, s->d_dict, sizeof(int32_t) * DF_DICT_WORDS, sizeof(int32_t) * DF_DICT_WORDS, false);
+    const size_t graph = s->d_graph.p ? std::min<size_t>(128 * (size_t)s->count, s->d_graph.cap) : 0;
+    if (e == cudaSuccess) e = clone_buf(segs, z->d_graph, s->d_graph, graph, graph, true);
+    if (e == cudaSuccess) e = clone_buf(segs, z->d_in, s->d_in, s->held() ? s->held() + 16 : 0, s->held(), true);
+    return e;
+}
+
+// the context's storage is copied by the caller: device storage in the call's launch, host storage by memcpy after it
+cudaError_t clone_context(const pngb200_png_context* s, pngb200_png_context* c, uint8_t* pixels, std::vector<CopySegment>& segs)
+{
+    c->ctx = s->ctx;
+    c->w = s->w, c->h = s->h, c->volume = s->volume, c->depth = s->depth;
+    c->interlaced = s->interlaced;
+    c->memspace = s->memspace;
+    c->pixels = pixels;
+    c->storage = s->storage, c->fsize = s->fsize;
+    c->copied = s->copied, c->drained = s->drained;
+    c->pass = s->pass, c->row = s->row;
+    c->terminal = s->terminal;
+    c->status = s->status, c->err_a = s->err_a, c->err_b = s->err_b;
+    c->band[0] = s->band[0], c->band[1] = s->band[1];
+    c->z = new pngb200_inflator();
+    cudaError_t e = clone_inflator(s->z, c->z, segs);
+    if (e == cudaSuccess) e = clone_buf(segs, c->d_filt, s->d_filt, s->fsize + 16, s->copied, false);
+    if (e == cudaSuccess && s->memspace == PNGB200_MEM_HOST) e = clone_buf(segs, c->d_img, s->d_img, s->storage, s->storage, false);
+    if (e == cudaSuccess && s->memspace == PNGB200_MEM_DEVICE && s->storage) segs.push_back({s->pixels, pixels, s->storage});
+    return e;
+}
+
+}  // namespace
 
 #include "png_file.cuh"
